@@ -49,6 +49,8 @@ def parse():
     ap.add_argument("--no-graph", action="store_true", help="launch kernels eagerly instead of replaying a CUDA graph")
     ap.add_argument("--gather-every", type=int, default=0, help="all-gather the detections every G steps (0: once, after the last step)")
     ap.add_argument("--no-nms-c5", action="store_true", help="skip the 100k-box NMS stress (BASELINE configs[4]) leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the detections of the last timed step to DIR/<name>.npy (float32)")
     args = ap.parse_args()
     args.wl = WORKLOADS[args.config]
     if args.batch is None:
@@ -78,7 +80,7 @@ def build_model(cfg, args):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -354,6 +356,17 @@ def nms_c5_leg(dev, hbm_peak):
     return out
 
 
+def dump_outputs(out_dir, packed):
+    """What a caller of the timed path receives for the last step: the packed detections [B, D, box + score + label +
+    valid] as they landed on the host, split into named float32 arrays (the seeded clouds make them reproducible)."""
+    import numpy as np
+
+    det = packed.numpy().astype(np.float32)
+    os.makedirs(out_dir, exist_ok=True)
+    for name, arr in (("boxes", det[..., :-3]), ("scores", det[..., -3]), ("labels", det[..., -2]), ("valid", det[..., -1])):
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(arr))
+
+
 def main():
     args = parse()
     _claim_stdout()
@@ -488,6 +501,8 @@ def main():
     sampler.mark()                      # clocks are sampled from here to the end of the per-kernel pass (same load)
     ms = timed(step_device, args.steps, False)
     ms_e2e = timed(step_e2e, args.steps, True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, state["out_pinned"].view(B, -1, state["out_pinned"].shape[-1]))
 
     # ---- per-stage pass: eager launches of the SAME kernels, CUDA events around every det3d_b200 call on the
     #      launching stream (voxelize / rulebook / sparse convs / dense convs / predict): launch count + rooflines ----
@@ -544,15 +559,11 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except OSError:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    bf16_peak = float(peaks.get("bf16_tflops", 1590.0))
-    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback (B200_PROFILING.md)"
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    bf16_peak = float(peaks.get("bf16_tflops", 989.0))
+    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback (H100 SXM data sheet: 3.35 TB/s, 989 TFLOP/s dense BF16)"
     traffic = {}
-    try:      # dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` captures
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))
-    except OSError:
-        pass
-    traffic_note = "static: from the committed ncu --set full capture (profiles/r2_traffic.json), not measured by this run"
+    traffic_note = "DRAM traffic is not measured by this run"
     ms_step = ms / args.steps
     st_ms, st_cnt = stage_ms(events, n_prof)
     timing = "CUDA events around each call on its launching stream, eager pass of %d steps" % n_prof
@@ -587,9 +598,9 @@ def main():
         tf = flops / (launch_ms * 1e-3) / 1e12
         per_math = 3.0 if args.math == "fp16x3" else 6.0       # bf16-peak-equivalents spent per fp32-equivalent flop
         rooflines["roofline"] = {
-            "kernel": ("d3b::bev_conv16_cs_kernel (channel-stationary M128 x N256 tiles): dense BEV conv3x3 %d->%d (RPN), %d launches/step"
+            "kernel": ("d3b::bev_conv16_cs_kernel (channel-stationary, C_out x 256-pixel tiles): dense BEV conv3x3 %d->%d (RPN), %d launches/step"
                        % (key[0], key[1], d["n"] // n_prof)
-                       if ((_lib.lib().d3b_get_bev_variant() == 1 or (_lib.lib().d3b_get_bev_variant() == 2 and d["info"].get("tiles", 0) >= 296))
+                       if (_lib.lib().d3b_get_bev_variant() == 1
                            and key[2] == 1 and key[1] % 128 == 0 and key[0] % 64 == 0) else
                        "d3b::bev_conv16_kernel<3,%d,%d>: dense BEV conv3x3 %d->%d (RPN), %d launches/step"
                        % (key[2], min(key[1], 128), key[0], key[1], d["n"] // n_prof)) if args.math == "fp16x3" else

@@ -4,7 +4,7 @@ Det3D configs and user code import `det3d.builder`, `det3d.utils.config_tool`,
 `det3d.models...`, `det3d.core.input.voxel_generator`, ... (e.g.
 examples/second/configs/kitti_car_vfev3_spmiddlefhd_rpn1_mghead_syncbn.py:4-5).  This
 package makes every `det3d.<path>` resolve to the SAME module object as
-`det3d_b200.<path>`, so those imports work unchanged against the B200-native
+`det3d_b200.<path>`, so those imports work unchanged against the H100-native
 implementation.
 """
 import importlib

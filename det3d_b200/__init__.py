@@ -1,4 +1,4 @@
-"""det3d_b200: B200-native (sm_100a) point-cloud inference hot path behind Det3D's module API.
+"""det3d_b200: H100-native (sm_90a) point-cloud inference hot path behind Det3D's module API.
 
 voxelize -> sparse 3-D conv middle encoder -> rotated-box IoU/NMS, as hand-written
 CUDA behind a C ABI (include/det3d_b200.h).  The sub-packages mirror the

@@ -1,9 +1,9 @@
-"""In-tree nvcc build of the det3d_b200 C-ABI library (sm_100a only).
+"""In-tree nvcc build of the det3d_b200 C-ABI library (sm_90a only: H100).
 
 `python -m det3d_b200.build` (or `__graft_entry__.build()`) cross-compiles
 every CUDA translation unit under `det3d_b200/csrc/` into
-`det3d_b200/lib/libdet3d_b200.so`.  The library is git-ignored but travels to
-the GPU box with the repo snapshot; nothing is JIT-compiled at import time.
+`det3d_b200/lib/libdet3d_b200.so`.  The library is a git-ignored build product
+of the source tree; nothing is JIT-compiled at import time.
 """
 import hashlib
 import os
@@ -22,7 +22,7 @@ NVCC_FLAGS = [
     "-O3",
     "-std=c++17",
     "-gencode",
-    "arch=compute_100a,code=sm_100a",
+    "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-Xcompiler",
     "-fPIC",

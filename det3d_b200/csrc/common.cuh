@@ -1,4 +1,4 @@
-// Shared helpers for the det3d_b200 CUDA translation units (sm_100a only).
+// Shared helpers for the det3d_b200 CUDA translation units (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -71,13 +71,13 @@ int nms_batched(int fmt_kernel, const float* boxes, int n_cap, const int* n_dev,
 // ---- programmatic dependent launch --------------------------------------------------------------------------------
 // The convolution kernels run back to back on one stream.  Launched with programmatic stream serialisation, kernel N+1 is
 // scheduled as soon as every CTA of kernel N has executed `griddepcontrol.launch_dependents` (they do so on entry): its
-// launch latency and its prologue (barrier init, TMEM allocation, rulebook staging -- nothing that reads kernel N's
+// launch latency and its prologue (barrier init, rulebook staging -- nothing that reads kernel N's
 // output) overlap kernel N's tail; `griddepcontrol.wait` (executed by every thread before it touches activations) then
 // blocks until kernel N has completed and its writes are visible.  Inside a captured CUDA graph the edge becomes a
 // programmatic dependency.  d3b_set_pdl(0) turns it off (plain stream order).
 bool pdl_enabled();
-// bevconv16_sm100.cu: 0 = pixel-stationary tiles (two M128 halves) everywhere, 1 = channel-stationary N256 kernel for the
-// 3x3 stride-1 128-channel-block layers, 2 = channel-stationary when a CTA walks several tiles (d3b_set_bev_variant)
+// bevconv16_sm90.cu: 0 = pixel-stationary tiles (two 128-pixel halves) everywhere, 1 = channel-stationary kernel for the
+// 3x3 stride-1 128-channel-block layers, 2 = automatic = pixel-stationary, the faster one on the H100 (d3b_set_bev_variant)
 int bev_variant();
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_maybe_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
@@ -98,12 +98,12 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
 __device__ __forceinline__ void pdl_wait_prior_grid() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // ---- device constants --------------------------------------------------------
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 static inline int div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 // Grid for a grid-stride kernel over `n` items: enough CTAs to cover n but
-// never more than `waves` full waves of the 148 SMs at `ctas_per_sm`.
+// never more than `waves` full waves of the 132 SMs at `ctas_per_sm`.
 static inline int grid_for(long long n, int block, int ctas_per_sm = 8) {
   long long want = (n + block - 1) / block;
   long long cap = (long long)kNumSMs * ctas_per_sm;

@@ -14,7 +14,7 @@
 //       corners in fp32 exactly as box_np_ops.py:419-497 builds them, polygon
 //       clipping in fp64.
 //
-// B200 design: (1) the N x N/64 suppression bitmask is produced for the upper
+// Design: (1) the N x N/64 suppression bitmask is produced for the upper
 // triangle only (the sweep never reads the rest) by one thread per row box,
 // with an exact-safe disjoint-circle test in front of the ~2k-instruction
 // polygon routine; (2) the greedy sweep runs on the device (one CTA, `remv`

@@ -12,7 +12,7 @@
 //
 // This variant serves the layers the tensor-core kernel does not take (C_in
 // not a multiple of 8, e.g. the 4/5-channel input layer) and is the
-// in-library cross-check of the tcgen05 kernel.
+// in-library cross-check of the tensor-core kernel.
 #include "common.cuh"
 
 namespace d3b {

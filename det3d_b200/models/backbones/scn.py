@@ -1,4 +1,4 @@
-"""Sparse middle encoders SpMiddleFHD / SpMiddleResNetFHD on the B200 kernels.
+"""Sparse middle encoders SpMiddleFHD / SpMiddleResNetFHD on the H100 kernels.
 
 Same registry names, constructor signatures, `middle_conv` parameter layout
 (state_dict keys `middle_conv.<idx>.{weight,bias,running_mean,...}`, SURVEY App. A.3)

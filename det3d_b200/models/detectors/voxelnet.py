@@ -34,7 +34,7 @@ class SingleStageDetector(nn.Module):
 class _FusedBevMixin:
     """Routes RPN + heads through the det3d_b200 tensor-core kernels.
 
-    math = "fp16x3" (default): NHWC split-f16 planes + TMA tensor maps (csrc/bevconv16_sm100.cu), any RPN the
+    math = "fp16x3" (default): NHWC split-f16 planes + TMA tensor maps (csrc/bevconv16_sm90.cu), any RPN the
     reference builds; "tf32x3": the round-1 gather kernel (stride-1 RPN only), which is also where a forward is
     re-run when a feature leaves the f16 range (`overflow_flag`)."""
     use_fused_bev = True

@@ -1,4 +1,4 @@
-"""B200-native stand-in for the `spconv` (v1.x) package surface Det3D uses."""
+"""H100-native stand-in for the `spconv` (v1.x) package surface Det3D uses."""
 from .core import (ConvWeights, Rulebook, SparseLevel, build_conv_rulebook, build_subm_rulebook,
                    alloc_conv_rulebook, alloc_subm_rulebook, level_from_coors, sparse_conv,
                    sparse_to_dense, force_algo)

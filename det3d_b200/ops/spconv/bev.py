@@ -5,7 +5,7 @@ followed by BN2d + ReLU, then a 1x1 "deblock") and the MultiGroupHead 1x1 convs
 (det3d/models/bbox_heads/mg_head.py:198-230) are dense stride-1 convolutions over the
 [B, 200, 176] BEV grid.  In channels-last layout a dense conv IS the gather-GEMM the sparse
 kernel already performs, with a static rulebook (d3b_rulebook_dense2d: neighbour = row +- 1,
-+- W, -1 at the border = zero padding).  So the same tcgen05 3xTF32 kernel -- fp32-equivalent
++- W, -1 at the border = zero padding).  So the same tensor-core 3xTF32 kernel -- fp32-equivalent
 accuracy, BN/ReLU folded into its epilogue -- replaces fp32 cuDNN here, and the head's three
 1x1 convs become ONE conv whose [B*H*W, 32] output rows are already the NHWC-permuted layout
 `Head.forward` produces with `.permute(0, 2, 3, 1)`.
@@ -186,7 +186,7 @@ class FusedBevStackTF32:
 
 # ======================================================================================================
 # FP16x3 path: the whole RPN (any block strides / ConvTranspose deblocks / concat) + all task heads on
-# NHWC f16 planes through TMA tensor maps (csrc/bevconv16_sm100.cu).
+# NHWC f16 planes through TMA tensor maps (csrc/bevconv16_sm90.cu).
 # ======================================================================================================
 from . import conv16  # noqa: E402
 

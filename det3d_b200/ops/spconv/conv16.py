@@ -2,8 +2,8 @@
 
 An activation is carried as two f16 planes, hi = f16(x) and lo = f16(x - hi) (`Planes`); weights are split the same
 way after an exact power-of-two scaling.  `sparse_conv16` is the output-stationary sparse convolution
-(csrc/spconv16_sm100.cu: deterministic, fused bias/BN/residual/ReLU epilogue), `BevConv16` a dense NHWC 3x3 / 1x1 /
-ConvTranspose layer through TMA tensor maps (csrc/bevconv16_sm100.cu).
+(csrc/spconv16_sm90.cu: deterministic, fused bias/BN/residual/ReLU epilogue), `BevConv16` a dense NHWC 3x3 / 1x1 /
+ConvTranspose layer through TMA tensor maps (csrc/bevconv16_sm90.cu).
 
 Reference call sites: det3d/models/backbones/scn.py:106-157,323-355 (sparse levels),
 det3d/models/necks/rpn.py:82-159 and det3d/models/bbox_heads/mg_head.py:198-230 (dense BEV).
@@ -62,7 +62,7 @@ class Planes:
 
 
 def supported(c_in, c_out):
-    """Shapes the tcgen05 FP16x3 sparse kernel takes (first layers with a handful of fp32 channels run on the
+    """Shapes the wgmma FP16x3 sparse kernel takes (first layers with a handful of fp32 channels run on the
     fp32-input variant instead)."""
     return c_in % 8 == 0 and 8 <= c_in <= 512 and c_out in (16, 32, 64, 128)
 

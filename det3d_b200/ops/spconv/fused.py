@@ -79,7 +79,7 @@ class FusedSparseEncoder:
     def __init__(self, middle_conv):
         self.plan = compile_plan(middle_conv)
         self._state = None
-        # "fp16x3" (default): output-stationary tcgen05 kernels on split-f16 planes (csrc/spconv16_sm100.cu) --
+        # "fp16x3" (default): output-stationary wgmma kernels on split-f16 planes (csrc/spconv16_sm90.cu) --
         # deterministic, fused epilogues, no atomics.  "tf32x3": the round-1 kernels (pair-based + fp32 atomics, or
         # output-stationary with deterministic=True); also the fallback when a feature leaves the f16 range.
         self.math = "fp16x3"

@@ -1,5 +1,5 @@
 /*
- * det3d_b200 -- C ABI of the B200-native point-cloud inference hot path.
+ * det3d_b200 -- C ABI of the H100-native (sm_90a) point-cloud inference hot path.
  *
  * Every entry point is `extern "C"`, takes plain pointers / sizes / a CUDA
  * stream (as void*), returns an int status (0 = D3B_OK), never calls exit(),
@@ -40,9 +40,9 @@ unsigned long long d3b_launch_count(void);
  * launch latency and prologue overlap the previous kernel's tail; results are unaffected. 0 = plain stream order. */
 void d3b_set_pdl(int on);
 /* Schedule of d3b_bev_conv16 for 3x3 stride-1 layers whose output blocks are 128 channels wide (the RPN blocks of
- * necks/rpn.py:124-142): 0 = pixel-stationary (two M128 x N128 halves per 16 x 16 pixel tile), 1 = channel-stationary
- * (C_out on the TMEM lanes, one M128 x N256 MMA covers the tile), 2 = automatic (default: channel-stationary when the
- * launch has at least two tiles per SM).  Same products in the same order: the results are bit-identical. */
+ * necks/rpn.py:124-142): 0 = pixel-stationary (two 128-pixel halves per 16 x 16 pixel tile), 1 = channel-stationary
+ * (C_out as the wgmma M dimension, the 256 tile pixels as N), 2 = automatic (default: pixel-stationary, measured the
+ * faster schedule on the H100).  Same products in the same order: the results are bit-identical. */
 void d3b_set_bev_variant(int variant);
 int d3b_get_bev_variant(void);
 
@@ -156,8 +156,8 @@ int d3b_rulebook_conv(const int32_t* in_coors, const int32_t* n_in, int32_t in_c
  *                    + residual[o,:] )
  * ========================================================================= */
 #define D3B_ALGO_SIMT 0     /* fp32 FFMA, output-stationary                              */
-#define D3B_ALGO_TC 1       /* tcgen05 3xTF32 (fp32-equivalent), output-stationary tiles  */
-#define D3B_ALGO_TC_PAIRS 2 /* tcgen05 3xTF32 over compacted rulebook pairs (per offset:  */
+#define D3B_ALGO_TC 1       /* wgmma 3xTF32 (fp32-equivalent), output-stationary tiles    */
+#define D3B_ALGO_TC_PAIRS 2 /* wgmma 3xTF32 over compacted rulebook pairs (per offset:    */
                             /* dense chunks of 128 valid pairs), fp32 atomics into feat_out */
 
 typedef struct {

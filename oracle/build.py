@@ -22,7 +22,8 @@ def build(force=False):
         subprocess.run(["make", "-C", HERE, "liboracle.so"] + (["-B"] if force else []), check=True,
                        stdout=subprocess.DEVNULL)
     ref_src = "/root/reference/det3d/ops/iou3d/src/iou3d_kernel.cu"
-    if os.path.exists(ref_src) and (force or not os.path.exists(REF_LIB)):
+    # rebuilt when the recipe (architecture flags) changed, not only when missing: an image for another GPU does not load
+    if os.path.exists(ref_src) and (force or _stale(REF_LIB, [ref_src, os.path.join(HERE, "Makefile")])):
         subprocess.run(["make", "-C", HERE, "ref"], check=True, stdout=subprocess.DEVNULL)
     build_ref_voxel(force)
     return LIB

@@ -1,7 +1,7 @@
-"""bench.py JSON lines -> profiles/r2_results.md (the table DESIGN.md section 9 points to).
+"""bench.py JSON lines -> a markdown results table (printed to stdout).
 
-    python profiles/make_results.py profiles/r2_bench_second.json profiles/r2_bench_pillars.json profiles/r2_bench_cbgs.json \
-        [--scale profiles/r2_scale_second_n1.json profiles/r2_scale_second_n2.json ...] > profiles/r2_results.md
+    python profiles/make_results.py profiles/h100_bench_second.json profiles/h100_bench_pillars.json profiles/h100_bench_cbgs.json \
+        [--scale <torchrun N = 1 line> <N = 2 line> ...]
 """
 import json
 import sys
@@ -18,7 +18,8 @@ def main():
     if "--scale" in args:
         i = args.index("--scale")
         args, scale = args[:i], args[i + 1:]
-    out = ["# Round 2 results (B200, `bench.py`, synthetic clouds, CUDA-graph replay, L2 flushed between steps)", ""]
+    out = ["# Results (`bench.py`, synthetic clouds, CUDA-graph replay, L2 flushed between steps; GPU and power limit: "
+           "profiles/README.md)", ""]
     out += ["| config | workload | clouds/s (device) | ms/step | clouds/s (e2e, host buffers) | launches/step | SM clock |",
             "|---|---|---|---|---|---|---|"]
     rows = [load(p) for p in args]

@@ -9,11 +9,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 GOLDEN = os.path.join(ROOT, "tests", "golden")
-REFERENCE = "/root/reference"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: the kernels are built for sm_90a)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -44,7 +43,3 @@ def golden_voxel_cases():
 
 def load_golden(name):
     return dict(np.load(os.path.join(GOLDEN, name + ".npz")))
-
-
-def has_reference():
-    return os.path.isdir(REFERENCE)

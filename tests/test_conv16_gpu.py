@@ -1,5 +1,5 @@
-"""Split-f16 ("FP16x3") tcgen05 convolutions vs fp32 references (the plain-PyTorch fp32 restatement of the op):
-csrc/spconv16_sm100.cu (sparse, output-stationary, deterministic) and csrc/bevconv16_sm100.cu (dense NHWC via TMA)."""
+"""Split-f16 ("FP16x3") wgmma convolutions vs fp32 references (the plain-PyTorch fp32 restatement of the op):
+csrc/spconv16_sm90.cu (sparse, output-stationary, deterministic) and csrc/bevconv16_sm90.cu (dense NHWC via TMA)."""
 import numpy as np
 import pytest
 import torch
@@ -174,7 +174,7 @@ def test_bev_conv16_transpose_into_concat_slice(up, c_in, c_out, h, w):
     (5, 64, 48, 128, 128),        # more tiles than SMs: CTAs walk several tiles (buffer / stage parities carry over)
 ])
 def test_bev_conv16_channel_stationary_variant(b, h, w, c_in, c_out):
-    """d3b_set_bev_variant(1): the transposed schedule (C_out on the TMEM lanes, one N = 256 MMA per 16 x 16 pixel tile)
+    """d3b_set_bev_variant(1): the transposed schedule (C_out as the wgmma M dimension, the tile's pixels as N)
     against float64 conv2d and against the pixel-stationary schedule (same products, same order, same chains)."""
     from det3d_b200 import _lib
     from det3d_b200.ops.spconv import conv16

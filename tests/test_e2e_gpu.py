@@ -178,7 +178,7 @@ def test_model_predict_api(setup):
 
 
 def test_fused_bev_path_matches_cudnn_path(setup):
-    """RPN + heads through the channels-last tcgen05 kernels vs the module's torch/cuDNN fp32 forward."""
+    """RPN + heads through the channels-last wgmma kernels vs the module's torch/cuDNN fp32 forward."""
     from det3d_b200.utils.synthetic import lidar_like_cloud
     cfg, pipe, cpu = setup
     model = pipe.model

@@ -1,14 +1,13 @@
 """The reference's dataset-side boundary (SURVEY 2.1 #16, 8a4): `Voxelization`, `AssignTarget`, `Reformat`, `Compose`
 (det3d/datasets/pipelines/) and `collate_kitti` (det3d/torchie/parallel/collate.py:90-150) under their own names."""
-import ast
-import collections
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from conftest import REFERENCE, ROOT, has_reference
+from boundary_golden import flatten, load_flat, reference_config
+from conftest import ROOT
 
 STOCK = [
     "examples/second/configs/kitti_car_vfev3_spmiddlefhd_rpn1_mghead_syncbn.py",
@@ -17,14 +16,13 @@ STOCK = [
 ]
 
 
-@pytest.mark.skipif(not has_reference(), reason="reference checkout not present")
 @pytest.mark.parametrize("rel", STOCK)
 def test_stock_test_pipeline_builds(rel):
-    """cfg.test_pipeline of an UNMODIFIED reference config builds through PIPELINES (every step is registered)."""
+    """cfg.test_pipeline of an UNMODIFIED reference config (as the reference's file parses, tests/golden/
+    reference_configs.json.gz) builds through PIPELINES (every step is registered)."""
     from det3d.datasets.pipelines import Compose
-    from det3d.torchie import Config
 
-    cfg = Config.fromfile(os.path.join(REFERENCE, rel))
+    cfg = reference_config(rel)
     pipe = Compose(cfg.test_pipeline)
     names = [type(t).__name__ for t in pipe.transforms]
     assert names == ["LoadPointCloudFromFile", "LoadPointCloudAnnotations", "Preprocess", "Voxelization", "AssignTarget",
@@ -63,37 +61,22 @@ def _sample(i, n_vox, max_pts=5, ndim=4, n_anchor=12):
     )
 
 
-def _reference_collate():
-    """The reference function itself, lifted out of its module (whose package imports do not resolve here)."""
-    src = open(os.path.join(REFERENCE, "det3d/torchie/parallel/collate.py")).read()
-    fn = next(n for n in ast.parse(src).body if isinstance(n, ast.FunctionDef) and n.name == "collate_kitti")
-    ns = dict(np=np, torch=torch, collections=collections, defaultdict=collections.defaultdict)
-    exec(compile(ast.Module(body=[fn], type_ignores=[]), "collate.py", "exec"), ns)
-    return ns["collate_kitti"]
+COLLATE_BATCH = (7, 0, 13)        # voxels per sample of the batch the reference collate_kitti was run on
 
 
-def _same(a, b):
-    if isinstance(a, dict):
-        return set(a) == set(b) and all(_same(a[k], b[k]) for k in a)
-    if isinstance(a, (list, tuple)):
-        return len(a) == len(b) and all(_same(x, y) for x, y in zip(a, b))
-    if torch.is_tensor(a):
-        return torch.is_tensor(b) and a.dtype == b.dtype and a.shape == b.shape and torch.equal(a, b)
-    if isinstance(a, np.ndarray):
-        return isinstance(b, np.ndarray) and a.dtype == b.dtype and np.array_equal(a, b)
-    return a == b
-
-
-@pytest.mark.skipif(not has_reference(), reason="reference checkout not present")
 def test_collate_kitti_equals_reference_function():
+    """collate_kitti == the reference's collate_kitti (its output on this batch: tests/golden/collate_kitti_reference.npz)
+    in structure, container and element types, dtypes, shapes and every bit."""
     from det3d.torchie.parallel import collate_kitti
 
-    batch = [_sample(i, n) for i, n in enumerate((7, 0, 13))]
-    want = _reference_collate()(batch)
+    batch = [_sample(i, n) for i, n in enumerate(COLLATE_BATCH)]
+    want_arrays, want_kinds = load_flat("collate_kitti_reference.npz")
     got = collate_kitti(batch)
-    assert set(got) == set(want)
-    for k in want:
-        assert _same(got[k], want[k]), k
+    got_arrays, got_kinds = flatten(got)
+    assert got_kinds == want_kinds
+    assert set(got_arrays) == set(want_arrays)
+    for k, a in want_arrays.items():
+        assert got_arrays[k].dtype == a.dtype and np.array_equal(got_arrays[k], a), k
     assert got["coordinates"][:, 0].tolist() == [0] * 7 + [2] * 13
     with pytest.raises(NotImplementedError):
         collate_kitti([dict(labels=[np.zeros(3)])])

@@ -6,7 +6,8 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import REFERENCE, ROOT, has_reference, load_golden
+from boundary_golden import reference_config
+from conftest import ROOT, load_golden
 
 
 def test_registry_semantics():
@@ -61,7 +62,6 @@ def test_shipped_config_builds_second():
     assert tuple(sd["neck.blocks.0.1.weight"].shape) == (128, 128, 3, 3)
 
 
-@pytest.mark.skipif(not has_reference(), reason="reference checkout not present")
 @pytest.mark.parametrize("rel", [
     "examples/second/configs/kitti_car_vfev3_spmiddlefhd_rpn1_mghead_syncbn.py",
     "examples/cbgs/configs/nusc_all_vfev3_spmiddleresnetfhd_rpn2_mghead_syncbn.py",
@@ -71,7 +71,7 @@ def test_reference_config_loads_unchanged(rel):
     from det3d.models import build_detector
     from det3d.torchie import Config
 
-    cfg = Config.fromfile(os.path.join(REFERENCE, rel))
+    cfg = reference_config(rel)           # the reference's own file as Config.fromfile parses it (tests/golden)
     model = build_detector(cfg.model, train_cfg=None, test_cfg=cfg.test_cfg)
     if "point_pillars" in rel:
         assert type(model).__name__ == "PointPillars"

@@ -76,7 +76,7 @@ def main():
         rows.append(("C5 iou3d NMS, 100k %s boxes, thr %.1f" % (kind, thr), "%.1f ms" % ms,
                      "%.2e pair tests/s; mask 1.25 GB stays on the device" % (100000 * 99999 / 2 / (ms * 1e-3))))
 
-    print("# r1: timings of the other BASELINE configurations (B200, CUDA events, inputs resident)\n")
+    print("# r1: timings of the other BASELINE configurations (H100, CUDA events, inputs resident)\n")
     print("| configuration | time | note |\n|---|---|---|")
     for r in rows:
         print("| %s | %s | %s |" % r)
