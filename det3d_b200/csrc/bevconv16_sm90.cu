@@ -15,9 +15,9 @@
 //  * FP16x3: per k-step three MMAs (A_lo.B_hi, A_hi.B_lo, A_hi.B_hi) with fp32 accumulation in registers -- but only
 //    across ONE kernel offset (<= 12 MMAs) into a fresh partial: the tensor core truncates on every accumulation, and
 //    chaining all 216 MMAs of a 3x3x128 reduction into one accumulator shrinks the outputs in proportion to the chain
-//    length, which 20 layers turn into > 1e-4.  The partial is scaled by 1 + n * 2^-26 (the mean truncation of its
-//    n MMAs) and added into the running fp32 sums with round-to-nearest; at the end of the tile the epilogue applies
-//    bias / BN / ReLU and writes the f16 planes.
+//    length, which 20 layers turn into > 1e-4.  The partial is added into the running fp32 sums with round-to-nearest;
+//    at the end of the tile the epilogue scales the sums by 1 + n * 2^-26 (the mean truncation of n MMAs, gmma.cuh),
+//    applies bias / BN / ReLU and writes the f16 planes.
 //  * Warp roles: 8 consumer warps (wgmma + epilogue), 1 TMA warp; A ring of 2 stages (4 patches each), B ring of 2..4
 //    stages, all mbarrier-driven; persistent grid.
 //  * stride 2 (RPN down-sampling blocks): the box is loaded with elementStrides = 2, one load per (ky, kx).
@@ -38,6 +38,7 @@ struct BvEpi {          // same fields as spconv16_sm90.cu (kept local: the two 
   const float* scale;
   const float* shift;
   float acc_scale;
+  float corr;           // mean truncation of the layer's partials (gmma.cuh), applied to the sums
   int relu;
 };
 
@@ -79,8 +80,6 @@ __device__ __forceinline__ uint32_t bv_pack_half2(__half a, __half b) {
   return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
 }
 
-// mean truncation of one partial: three MMAs per k-step of one (kernel offset, 64-channel slice)
-__device__ __forceinline__ float bv_trunc_fix(int n_ks) { return 1.f + 3.f * (float)n_ks * kTruncLossPerMma; }
 
 template <int KS, int STRIDE, int COUT>
 __global__ void __launch_bounds__(kBvThreads, 1)
@@ -183,7 +182,6 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
         for (int q = 0; q < COUT / 2; ++q) acc[m][q] = 0.f;
       for (int kb = 0; kb < g.n_kb; ++kb) {
         const int n_ks = min(kBvKc / 16, (g.c_in - kb * kBvKc + 15) / 16);
-        const float f_fix = bv_trunc_fix(n_ks);
         for (int kx = 0; kx < KS; ++kx) {
           for (int ky0 = 0; ky0 < KS; ky0 += Cfg::kRowsPerAStage) {
             const int sa = a_it % kBvAStages;
@@ -221,7 +219,7 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
                   gmma_fence_regs(part);
 #pragma unroll
                   for (int q = 0; q < Cfg::kPassN / 2; ++q)
-                    acc[m][np * Cfg::kPassN / 2 + q] = fmaf(part[q], f_fix, acc[m][np * Cfg::kPassN / 2 + q]);
+                    acc[m][np * Cfg::kPassN / 2 + q] += part[q];
                 }
               }
               __syncwarp();
@@ -247,6 +245,8 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
           for (int jn = 0; jn < COUT / 8; ++jn) {
             const int col = jn * 8 + 2 * (lane & 3);
             float v0 = acc[m][4 * jn + 2 * h] * epi.acc_scale, v1 = acc[m][4 * jn + 2 * h + 1] * epi.acc_scale;
+            v0 = fmaf(v0, epi.corr, v0);
+            v1 = fmaf(v1, epi.corr, v1);
             if (epi.bias) {
               const float2 bb = __ldg(reinterpret_cast<const float2*>(epi.bias + pcol + col));
               v0 += bb.x; v1 += bb.y;
@@ -390,7 +390,6 @@ bev_conv16_cs_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
     // ===================== consumer warpgroups: warpgroup wg -> output channels [64 wg, 64 wg + 64) =====================
     pdl_wait_prior_grid();                              // (output buffers may still be read by earlier kernels)
     const int wg = warp >> 2, wq = warp & 3;
-    const float f_fix = bv_trunc_fix(kBvKc / 16);      // (C_in % 64 == 0: four k-steps per offset and slice)
     bool ovf = false;
     uint32_t a_it = 0, b_it = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -428,7 +427,7 @@ bev_conv16_cs_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
               gmma_wait();
               gmma_fence_regs(part);
 #pragma unroll
-              for (int q = 0; q < 32; ++q) acc[nh * 32 + q] = fmaf(part[q], f_fix, acc[nh * 32 + q]);
+              for (int q = 0; q < 32; ++q) acc[nh * 32 + q] += part[q];
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(b_empty(sb));
@@ -454,6 +453,7 @@ bev_conv16_cs_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
             const int p = jn * 8 + 2 * (lane & 3) + c;
             const int y = y0 + (p >> 4), x = x0 + (p & 15);
             float v = acc[4 * jn + 2 * h + c] * epi.acc_scale;
+            v = fmaf(v, epi.corr, v);
             if (epi.bias) v += e_bias;
             if (epi.scale) v = fmaf(v, e_scale, e_shift);
             if (epi.relu) v = fmaxf(v, 0.f);
@@ -529,6 +529,7 @@ static int launch_bev(const d3b_bev16_params* p, const BvGeom& g, cudaStream_t s
   if (st != D3B_OK) return st;
   BvEpi e;
   e.bias = p->bias; e.scale = p->scale; e.shift = p->shift; e.acc_scale = p->acc_scale; e.relu = p->relu;
+  e.corr = trunc_correction(p->c_in);
   const int n_tiles = g.batch * g.tiles_y * g.tiles_x * g.groups;
   const int grid = n_tiles < kNumSMs ? n_tiles : kNumSMs;
   D3B_CUDA(launch_maybe_pdl(bev_conv16_kernel<KS, STRIDE, COUT>, dim3(grid), dim3(kBvThreads), Cfg::kSmemBytes, stream, tm_hi,
@@ -549,6 +550,7 @@ static int launch_bev_cs(const d3b_bev16_params* p, const BvGeom& g, cudaStream_
   if (st != D3B_OK) return st;
   BvEpi e;
   e.bias = p->bias; e.scale = p->scale; e.shift = p->shift; e.acc_scale = p->acc_scale; e.relu = p->relu;
+  e.corr = trunc_correction(p->c_in);
   const int n_tiles = g.batch * g.tiles_y * g.tiles_x * g.groups;
   const int grid = n_tiles < kNumSMs ? n_tiles : kNumSMs;
   D3B_CUDA(launch_maybe_pdl(bev_conv16_cs_kernel, dim3(grid), dim3(kBwThreads), kBwSmemBytes, stream, tm_hi, tm_lo, g,

@@ -266,11 +266,21 @@ __device__ __forceinline__ void gmma_fence_regs(float (&d)[R]) {
 }
 
 // Expected relative loss of one truncating tensor-core accumulation: the tensor core adds a product sum into the fp32
-// accumulator rounding toward zero.  2^-26 per MMA chained into one accumulator is the mean signed error measured for the
-// previous generation's tensor core (tcgen05); it has NOT been re-measured for wgmma on the H100.  Kernels chain at most
-// 12 MMAs into a partial and scale it by 1 + n * 2^-26, so the correction is <= 1.8e-7 relative per partial either way;
-// with it, the forward passes stay within the 1e-4 checks of tests/test_e2e_gpu.py and tests/test_pillars.py on the H100.
+// accumulator rounding toward zero.  Measured for wgmma.m64nNk16.f32.f16.f16 on an H100 80GB HBM3 at a 400 W power limit
+// (tools/trunc_bias.py, profiles/h100_trunc_bias.txt): 1.0 x 2^-26 per MMA of a 12-MMA partial when activations or
+// weights have mixed signs (what the network feeds the kernels), 1.3 to 1.5 x 2^-26 with all-positive operands.
 constexpr float kTruncLossPerMma = 1.4901161e-8f;   // 2^-26
+
+// The FP16x3 kernels chain the n = 3 * n_ks MMAs of one (kernel offset, 64-channel slice) into a partial and add the
+// partials to the running sums with round-to-nearest; the epilogue then scales the sum by 1 + c, computed as
+// fmaf(v, c, v) (1 + 12 * 2^-26 is not an fp32 number: a factor would round to 1 + 16 * 2^-26).  c is the layer's mean
+// n * kTruncLossPerMma: 12 * 2^-26 when C_in (per slot) is a multiple of 64; a ragged last slice chains fewer MMAs and
+// is weighted by its channels.
+__host__ __device__ inline float trunc_correction(int c_slot) {
+  const int full = c_slot / 64, rest = c_slot - 64 * full;
+  const float n = (float)(12 * 64 * full + 3 * ((rest + 15) / 16) * rest) / (float)c_slot;
+  return n * kTruncLossPerMma;
+}
 
 // 4-D tiled TMA load (tensor map in kernel parameter space): box -> shared memory, completes on an mbarrier
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, int c0, int c1, int c2, int c3, uint32_t bar) {

@@ -24,8 +24,8 @@
 // Accumulation.  The tensor core adds every MMA's partial sum into the fp32 accumulator with truncation (round toward
 // zero), a systematic shrink that grows with the number of MMAs chained into one accumulator; chaining a whole 3x3x3
 // layer (up to 648 MMAs) into one accumulator puts the encoder output beyond 1e-4.  So the chain is bounded: the
-// products of one slot (<= 12 MMAs) go into a fresh register partial, which is scaled by 1 + n * 2^-26 (the mean
-// truncation of its n MMAs) and added into the running fp32 sums with round-to-nearest -- the summation structure of
+// products of one slot (<= 12 MMAs) go into a fresh register partial, which is added into the running fp32 sums with
+// round-to-nearest; the epilogue scales the sums by 1 + n * 2^-26 (the mean truncation of n MMAs, gmma.cuh) -- the summation structure of
 // the reference's per-offset GEMM + scatter-add, in a fixed order.  An absent neighbour contributes an exact zero
 // partial, so a row's bits depend on its own neighbourhood only.
 //
@@ -76,6 +76,7 @@ struct OsEpi {
   const __half* res_hi;
   const __half* res_lo;
   float acc_scale;
+  float corr;                     // mean truncation of the layer's partials (gmma.cuh), applied to the sums
   int relu;
   int seq;                        // launch counter of this translation unit (development traces only)
 };
@@ -151,6 +152,8 @@ __device__ __forceinline__ bool epilogue2(float v0, float v1, const OsEpi& e, si
                                           __half* out_lo, float* out_f32) {
   v0 *= e.acc_scale;
   v1 *= e.acc_scale;
+  v0 = fmaf(v0, e.corr, v0);
+  v1 = fmaf(v1, e.corr, v1);
   if (e.bias) {
     const float2 b = __ldg(reinterpret_cast<const float2*>(e.bias + col));
     v0 += b.x; v1 += b.y;
@@ -249,7 +252,6 @@ spconv_os16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ 
         const int s = it % Cfg::kStages;
         const uint32_t ph = (it / Cfg::kStages) & 1u;
         const int n_ks = min(kOsKc / 16, (c_eff - kb * kOsKc + 15) / 16);
-        const float f_fix = 1.f + 3.f * (float)n_ks * kTruncLossPerMma;   // three MMAs per live k-step chained per partial
         if (warp == 0 && lane == 0) D3B_STAMP(6, it);
         D3B_WAIT(full_bar(s), ph, 3);
         const uint32_t a_hi = smem_base + s * Cfg::kStageBytes + wg * 8192u;   // rows 64 wg .. 64 wg + 63
@@ -275,7 +277,7 @@ spconv_os16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ 
           gmma_wait();
           gmma_fence_regs(part);
 #pragma unroll
-          for (int q = 0; q < Cfg::kPassN / 2; ++q) acc[np * Cfg::kPassN / 2 + q] = fmaf(part[q], f_fix, acc[np * Cfg::kPassN / 2 + q]);
+          for (int q = 0; q < Cfg::kPassN / 2; ++q) acc[np * Cfg::kPassN / 2 + q] += part[q];
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(empty_bar(s));     // the gather group may refill this stage
@@ -534,6 +536,7 @@ static OsEpi epi_of(const d3b_conv16_params* p) {
   e.bias = p->bias; e.scale = p->scale; e.shift = p->shift;
   e.res_hi = (const __half*)p->residual_hi; e.res_lo = (const __half*)p->residual_lo;
   e.acc_scale = p->acc_scale; e.relu = p->relu;
+  e.corr = 0.f;                                   // (set by the tensor-core launch; the FFMA first layer is exact-sum)
   static std::atomic<int> launch_seq{0};
   e.seq = launch_seq.fetch_add(1, std::memory_order_relaxed);
   return e;
@@ -549,10 +552,12 @@ static int launch_os16(const d3b_conv16_params* p, const int32_t* nbr, const uin
   const int grid = n_tiles < kNumSMs ? (n_tiles > 0 ? n_tiles : 1) : kNumSMs;
   const int pack = os16_pack(p->c_in, p->k_vol);
   const int n_kb = pack > 1 ? 1 : (p->c_in + kOsKc - 1) / kOsKc;
+  OsEpi epi = epi_of(p);
+  epi.corr = trunc_correction(p->c_in * pack);
   D3B_CUDA(launch_maybe_pdl(spconv_os16_kernel<COUT>, dim3(grid), dim3(Cfg::kThreads), Cfg::kSmemBytes, stream,
                             (const __half*)p->in_hi, (const __half*)p->in_lo, (const int*)nbr, (const unsigned int*)tile_mask,
                             (const int*)n_out, (int)out_cap, (int)p->c_in, n_kb, pack, (int)p->k_vol,
-                            (const __half*)p->weight_packed, epi_of(p),
+                            (const __half*)p->weight_packed, epi,
                             (__half*)p->out_hi, (__half*)p->out_lo, p->out_f32, (int*)p->overflow));
   D3B_LAUNCH_CHECK();
   return D3B_OK;

@@ -170,7 +170,8 @@ def sparse_to_bev16(x, level, out):
 class BevConv16:
     """One dense NHWC layer: Conv2d 3x3 (stride 1 / 2) or 1x1, or ConvTranspose2d(kernel = stride = up), with folded
     BatchNorm / bias / ReLU.  Output channels wider than 128 run as `cgroups` blocks of one launch; the result can land in
-    a channel slice [out_c0, out_c0 + C_out) of a wider (concat) buffer."""
+    a channel slice [out_c0, out_c0 + C_out) of a wider (concat) buffer when C_out is a whole number of blocks (32, 64,
+    128 or a multiple of 128); other widths are written with their zero padding into a buffer of `c_out_padded` channels."""
 
     def __init__(self, weight, ksize, stride=1, pad=0, up=1, bias=None, scale=None, shift=None, relu=False, device=None):
         # weight: [up*up, K*K, C_in, C_out] f32 (up*up = 1 for plain convs)
@@ -203,7 +204,9 @@ class BevConv16:
         for ug in range(ugroups):
             for cg in range(self.cgroups):
                 blk = w[ug, :, :, cg * self.c_blk:(cg + 1) * self.c_blk].contiguous()
-                images.append(pack_weight16(blk, w_exp)[0])
+                # one image per tap: the dense kernel reads [tap][64-channel slice] and never packs several kernel
+                # offsets into one slot the way the sparse kernel does for C_in 16 / 32
+                images += [pack_weight16(blk[t:t + 1], w_exp)[0] for t in range(k_vol)]
         self.packed = torch.cat(images)
         self.w_exp = w_exp
         self.acc_scale = math.ldexp(1.0, -w_exp)
@@ -234,6 +237,12 @@ class BevConv16:
         shape = ref.shape
         assert tuple(shape[:3]) == (b, ho, wo), "output grid %s != %s" % (tuple(shape[:3]), (b, ho, wo))
         p.out_channels, p.out_c0 = int(shape[3]), int(out_c0)
+        if self.c_out_padded != self.c_out_total and (p.out_c0 != 0 or p.out_channels != self.c_out_padded):
+            # the epilogue writes whole blocks: the padded columns would land on the neighbouring channels
+            raise _lib.D3BError("BevConv16: C_out %d is padded to %d; write it into a buffer of exactly %d channels, "
+                                "not a channel slice [%d, %d) of %d" % (self.c_out_total, self.c_out_padded,
+                                                                        self.c_out_padded, p.out_c0,
+                                                                        p.out_c0 + self.c_out_total, p.out_channels))
         if out is not None:
             p.out_hi, p.out_lo = out.hi.data_ptr(), out.lo.data_ptr()
         if out_f32 is not None:
