@@ -21,6 +21,9 @@
 //  * Warp roles: 8 consumer warps (wgmma + epilogue), 1 TMA warp; A ring of 2 stages (4 patches each), B ring of 2..4
 //    stages, all mbarrier-driven; persistent grid.
 //  * stride 2 (RPN down-sampling blocks): the box is loaded with elementStrides = 2, one load per (ky, kx).
+//  * Conv2d(kernel = stride = s, pad 0), s in {2, 3, 4} (the deblock rpn.py builds for an up-sampling stride 1/s):
+//    the same strided loads with elementStrides = s -- box (8-1)*s+1 columns x (16-1)*s+1 rows, at most 29 x 61 --
+//    one A stage per (64 channels, kx, ky).  Output rows / columns past floor(H / s) are not formed, as in torch.
 //  * groups: several weight blocks over the same input in one launch -- C_out = 256 as two N = 128 passes, and
 //    ConvTranspose2d(k = s, stride = s) as s*s 1x1 convolutions whose epilogues write pixel (y*s + dy, x*s + dx)
 //    into a channel slice of the concat buffer.
@@ -58,7 +61,7 @@ struct BvCfg {
   static constexpr int kBBytes = 2 * COUT * 128;                                      // [B_hi rows | B_lo rows]
   static constexpr int kBStages = COUT >= 128 ? 2 : 4;
   static constexpr int kSmemBytes = kBvAStages * kAStageBytes + kBStages * kBBytes + 1024 + 256;
-  // with stride 1 one A stage serves the KS kernel rows of a (kx, kb); with stride 2 every (ky, kx) has its own
+  // with stride 1 one A stage serves the KS kernel rows of a (kx, kb); with stride > 1 every (ky, kx) has its own
   static constexpr int kRowsPerAStage = STRIDE == 1 ? KS : 1;
   // partials are computed in column passes of kPassN outputs (C_out = 128: two, so that sums + partial fit registers)
   static constexpr int kPassN = COUT >= 128 ? 64 : COUT;
@@ -569,9 +572,13 @@ extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
   D3B_REQUIRE(p && p->in_hi && p->in_lo && p->weight_packed, "d3b_bev_conv16: null argument");
   D3B_REQUIRE(p->batch >= 1 && p->h_in >= 1 && p->w_in >= 1 && p->c_in >= 16 && p->c_in % 16 == 0,
               "d3b_bev_conv16: bad input shape [%d,%d,%d,%d] (C_in must be a multiple of 16)", p->batch, p->h_in, p->w_in, p->c_in);
-  D3B_REQUIRE((p->ksize == 1 || p->ksize == 3) && (p->stride == 1 || p->stride == 2) && !(p->ksize == 1 && p->stride != 1),
-              "d3b_bev_conv16: ksize %d stride %d not built (3x3 s1/s2, 1x1 s1)", p->ksize, p->stride);
-  D3B_REQUIRE(p->pad >= 0 && p->pad <= p->ksize / 2 + 1, "d3b_bev_conv16: pad %d", p->pad);
+  // kernel = stride = s (2..4): the strided Conv2d deblock; it tiles the input exactly, so it takes no padding
+  const bool k_is_s = p->ksize == p->stride && p->ksize >= 2 && p->ksize <= 4;
+  D3B_REQUIRE(k_is_s || ((p->ksize == 1 || p->ksize == 3) && (p->stride == 1 || p->stride == 2) &&
+                         !(p->ksize == 1 && p->stride != 1)),
+              "d3b_bev_conv16: ksize %d stride %d not built (3x3 s1/s2, 1x1 s1, k = s in {2, 3, 4})", p->ksize, p->stride);
+  D3B_REQUIRE(k_is_s ? p->pad == 0 : (p->pad >= 0 && p->pad <= p->ksize / 2 + 1),
+              "d3b_bev_conv16: pad %d not built for ksize %d stride %d", p->pad, p->ksize, p->stride);
   D3B_REQUIRE(p->up >= 1 && p->up <= 4 && p->cgroups >= 1 && p->groups == p->cgroups * p->up * p->up,
               "d3b_bev_conv16: groups %d != cgroups %d * up^2 (up %d)", p->groups, p->cgroups, p->up);
   D3B_REQUIRE((p->out_hi != nullptr) == (p->out_lo != nullptr) && (p->out_hi || p->out_f32),
@@ -580,6 +587,9 @@ extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
   D3B_REQUIRE(p->out_channels % 8 == 0 && p->out_c0 % 8 == 0 && p->out_c0 + p->cgroups * p->c_out <= p->out_channels,
               "d3b_bev_conv16: output channel slice [%d, %d) does not fit rows of %d", p->out_c0,
               p->out_c0 + p->cgroups * p->c_out, p->out_channels);
+  // (an input smaller than the kernel has no output; C division would round -1/s up to 0 and make one)
+  D3B_REQUIRE(p->h_in + 2 * p->pad >= p->ksize && p->w_in + 2 * p->pad >= p->ksize,
+              "d3b_bev_conv16: input %dx%d (pad %d) is smaller than the kernel %d", p->h_in, p->w_in, p->pad, p->ksize);
   BvGeom g;
   g.batch = p->batch;
   g.h_out = (p->h_in + 2 * p->pad - p->ksize) / p->stride + 1;
@@ -614,6 +624,9 @@ extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
   D3B_BEV_CASE(3, 1)
   D3B_BEV_CASE(3, 2)
   D3B_BEV_CASE(1, 1)
+  D3B_BEV_CASE(2, 2)
+  D3B_BEV_CASE(3, 3)
+  D3B_BEV_CASE(4, 4)
 #undef D3B_BEV_CASE
   set_error("d3b_bev_conv16: C_out per group %d not in {32, 64, 128}", p->c_out);
   return D3B_ERR_UNSUPPORTED;

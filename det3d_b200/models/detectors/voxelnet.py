@@ -51,6 +51,11 @@ class _FusedBevMixin:
             fused().math = math
 
     def overflow_flag(self, device):
+        # "cuda" (the pipeline's device) and "cuda:0" (a tensor's) must name the same flag: comparing them unresolved
+        # swapped in a fresh zero flag on every call, and the host never saw one the kernels had raised
+        device = torch.device(device)
+        if device.type == "cuda" and device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
         if self._ovf is None or self._ovf.device != device:
             self._ovf = torch.zeros(1, dtype=torch.int32, device=device)
         return self._ovf

@@ -227,8 +227,9 @@ def _layer16(conv, bn, relu, extra_pad, device):
 
 
 def rpn_is_fusable16(rpn):
-    """Every RPN the reference builds (necks/rpn.py:82-143): 3x3 blocks with stride 1 or 2, deblocks that are 1x1 convs
-    or ConvTranspose2d(kernel = stride); channel counts multiples of 16."""
+    """Every RPN the reference builds (necks/rpn.py:82-143): 3x3 blocks with stride 1 or 2; deblocks that are 1x1 convs,
+    ConvTranspose2d(kernel = stride <= 4), or Conv2d(kernel = stride = s, s in {2, 3, 4}, no padding / dilation /
+    groups: an up-sampling stride of 1/s, as in nuScenes PointPillars); channel counts multiples of 16."""
     try:
         for blk in rpn.blocks:
             for m in blk:
@@ -243,7 +244,10 @@ def rpn_is_fusable16(rpn):
                     if m.kernel_size != m.stride or m.stride[0] != m.stride[1] or m.stride[0] > 4 or m.in_channels % 16:
                         return False
                 elif isinstance(m, nn.Conv2d):
-                    if m.kernel_size != (1, 1) or m.stride != (1, 1) or m.in_channels % 16:
+                    s = m.stride[0]
+                    k_is_s = (m.kernel_size == m.stride == (s, s) and s in (2, 3, 4) and m.padding == (0, 0)
+                              and m.dilation == (1, 1) and m.groups == 1)
+                    if not (m.kernel_size == (1, 1) and m.stride == (1, 1) or k_is_s) or m.in_channels % 16:
                         return False
                 elif not isinstance(m, (nn.ReLU, nn.modules.batchnorm._BatchNorm)):
                     return False

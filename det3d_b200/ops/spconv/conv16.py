@@ -3,7 +3,7 @@
 An activation is carried as two f16 planes, hi = f16(x) and lo = f16(x - hi) (`Planes`); weights are split the same
 way after an exact power-of-two scaling.  `sparse_conv16` is the output-stationary sparse convolution
 (csrc/spconv16_sm90.cu: deterministic, fused bias/BN/residual/ReLU epilogue), `BevConv16` a dense NHWC 3x3 / 1x1 /
-ConvTranspose layer through TMA tensor maps (csrc/bevconv16_sm90.cu).
+kernel = stride / ConvTranspose layer through TMA tensor maps (csrc/bevconv16_sm90.cu).
 
 Reference call sites: det3d/models/backbones/scn.py:106-157,323-355 (sparse levels),
 det3d/models/necks/rpn.py:82-159 and det3d/models/bbox_heads/mg_head.py:198-230 (dense BEV).
@@ -168,10 +168,11 @@ def sparse_to_bev16(x, level, out):
 
 
 class BevConv16:
-    """One dense NHWC layer: Conv2d 3x3 (stride 1 / 2) or 1x1, or ConvTranspose2d(kernel = stride = up), with folded
-    BatchNorm / bias / ReLU.  Output channels wider than 128 run as `cgroups` blocks of one launch; the result can land in
-    a channel slice [out_c0, out_c0 + C_out) of a wider (concat) buffer when C_out is a whole number of blocks (32, 64,
-    128 or a multiple of 128); other widths are written with their zero padding into a buffer of `c_out_padded` channels."""
+    """One dense NHWC layer: Conv2d 3x3 (stride 1 / 2), 1x1, or kernel = stride = s (s in {2, 3, 4}, pad 0), or
+    ConvTranspose2d(kernel = stride = up), with folded BatchNorm / bias / ReLU.  Output channels wider than 128 run as
+    `cgroups` blocks of one launch; the result can land in a channel slice [out_c0, out_c0 + C_out) of a wider (concat)
+    buffer when C_out is a whole number of blocks (32, 64, 128 or a multiple of 128); other widths are written with their
+    zero padding into a buffer of `c_out_padded` channels."""
 
     def __init__(self, weight, ksize, stride=1, pad=0, up=1, bias=None, scale=None, shift=None, relu=False, device=None):
         # weight: [up*up, K*K, C_in, C_out] f32 (up*up = 1 for plain convs)

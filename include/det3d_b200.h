@@ -307,8 +307,11 @@ int d3b_sparse_to_bev16(const void* in_hi, const void* in_lo, const float* in_f3
                         const int32_t* n_rows, int32_t row_cap, int32_t channels, const int32_t spatial[3],
                         int32_t batch, void* out_hi, void* out_lo, void* stream);
 
-/* Dense NHWC convolution on planes [batch, h_in, w_in, c_in] through TMA tensor maps: 3x3 (stride 1 or 2) or 1x1,
- * zero padding `pad`, `groups` weight blocks of c_out (32/64/128) channels each in one launch:
+/* Dense NHWC convolution on planes [batch, h_in, w_in, c_in] through TMA tensor maps: 3x3 (stride 1 or 2) or 1x1
+ * with zero padding `pad` (<= ksize / 2 + 1), or ksize == stride == s for s in {2, 3, 4} with pad 0 (the Conv2d
+ * deblock of an up-sampling stride 1/s, necks/rpn.py:96-102; trailing rows / columns of an h_in or w_in that is not
+ * a multiple of s are not read, as in torch); other (ksize, stride, pad) return D3B_ERR_INVALID_ARG.
+ * `groups` weight blocks of c_out (32/64/128) channels each in one launch:
  *   group g -> channel block cg = g % cgroups, sub-pixel ug = g / cgroups, (uy, ux) = (ug / up, ug % up);
  *   conv output pixel (y, x) of group g is written to pixel (y*up + uy, x*up + ux) of the output tensor
  *   [batch, h_out*up, w_out*up, out_channels], channels [out_c0 + cg*c_out, out_c0 + (cg+1)*c_out).
