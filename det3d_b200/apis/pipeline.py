@@ -46,7 +46,7 @@ class InferencePipeline:
         self._anchors = [torch.from_numpy(a).to(self.device) for a in anchors]
         self._anchor_cache = {}
         self.strict_fp32 = strict_fp32
-        self._graphs = collections.OrderedDict()      # offsets tuple -> captured graph, least recently used first
+        self._graphs = collections.OrderedDict()      # (batch, bucket, ndim) -> _GraphEntry, least recently used first
         self.max_graphs = 8
         self._ovf_host = None
 
@@ -58,7 +58,9 @@ class InferencePipeline:
 
     @torch.no_grad()
     def forward_device(self, points, offsets):
-        """points [N_total, ndim] f32 on the device, offsets host list -> fixed-shape detections."""
+        """points [N_total, ndim] f32 on the device, offsets host list -> fixed-shape detections.
+
+        `offsets` may also be an int32 device tensor [B+1]; points.shape[0] is then a capacity (Voxelizer)."""
         batch = len(offsets) - 1
         vox = self.voxelizer(points, offsets)
         example = dict(
@@ -99,42 +101,79 @@ class InferencePipeline:
         self._graphs.clear()
         return True
 
-    @torch.no_grad()
-    def forward_graphed(self, points, offsets):
-        """forward_device + pack replayed from a CUDA graph (captured on first use per `offsets`).
+    @staticmethod
+    def bucket_of(n_points):
+        """Point capacity of the graph that serves a batch of n_points: the smallest power of two >= max(n, 1024)."""
+        return 1 << (max(int(n_points), 1024) - 1).bit_length()
 
-        Every stage has static shapes and device-resident counts, so the whole forward -- ~50
-        det3d_b200 launches plus the torch glue -- is one graph launch.  `points` may live on the
-        host (pinned) or the device; it is copied into the graph's static input buffer.
-        Returns the packed detections [B, D, nd+3] (a static buffer: consume before the next call)."""
-        key = tuple(int(o) for o in offsets)
+    @staticmethod
+    def check_offsets(offsets, n_points=None):
+        """Host-side validation of cloud offsets [0, n0, n0+n1, ...]: raises ValueError, before anything is enqueued."""
+        offsets = [int(o) for o in offsets]
+        if not 2 <= len(offsets) <= 65:
+            raise ValueError("offsets must hold batch + 1 entries with 1 <= batch <= 64, got %d" % len(offsets))
+        if offsets[0] != 0:
+            raise ValueError("offsets[0] must be 0, got %d" % offsets[0])
+        if any(b < a for a, b in zip(offsets[:-1], offsets[1:])):
+            raise ValueError("offsets must be non-decreasing: %s" % offsets)
+        if n_points is not None and offsets[-1] != n_points:
+            raise ValueError("offsets[-1] = %d but points has %d rows" % (offsets[-1], n_points))
+        return offsets
+
+    def _graph_entry(self, batch, n_points, ndim):
+        """The graph of (batch, bucket, ndim), least recently used last; a new entry has buffers but no graph yet."""
+        key = (batch, self.bucket_of(n_points), ndim)
         entry = self._graphs.get(key)
         if entry is not None:
             self._graphs.move_to_end(key)
-        if entry is None:
-            # One graph per distinct `offsets` (the per-cloud point counts are host arguments of d3b_voxelize).  Real
-            # LiDAR frames rarely repeat a point count: keep at most `max_graphs` graphs (LRU) so memory stays bounded;
-            # callers with free-running sizes should pad clouds to a few bucket sizes or use forward_device.
-            while len(self._graphs) >= self.max_graphs:
-                self._graphs.popitem(last=False)
-            static_pts = torch.zeros((key[-1], points.shape[1]), dtype=torch.float32, device=self.device)
-            static_pts.copy_(points)
+            return entry
+        while len(self._graphs) >= self.max_graphs:
+            self._graphs.popitem(last=False)
+        entry = self._graphs[key] = _GraphEntry(key[1], batch, ndim, self.device)
+        return entry
+
+    def _replay(self, entry, offsets):
+        """Make the graph's device offsets `offsets`, capture the graph on first use, replay.  The clouds must already
+        be in entry.points[:offsets[-1]]."""
+        key = tuple(offsets)
+        if entry.last_offsets != key:
+            # the pinned staging buffer may still feed the previous copy: wait for that one before rewriting it
+            entry.copied.synchronize()
+            entry.staging.numpy()[:] = key
+            entry.offsets.copy_(entry.staging, non_blocking=True)
+            entry.copied.record()
+            entry.last_offsets = key
+        if entry.graph is None:
             side = torch.cuda.Stream(device=self.device)
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
                 for _ in range(3):                      # warm-up: lazy buffers, weight packing, cuDNN plans
-                    self.pack(self.forward_device(static_pts, list(key)))
+                    self.pack(self.forward_device(entry.points, entry.offsets))
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                out = self.pack(self.forward_device(static_pts, list(key)))
+                entry.out = self.pack(self.forward_device(entry.points, entry.offsets))
                 _lib.graph_mark("end")          # (bench.py's in-graph stage timing; nothing unless _lib.GRAPH_MARKS is set)
-            entry = self._graphs[key] = (graph, static_pts, out)
-        graph, static_pts, out = entry
-        static_pts.copy_(points, non_blocking=True)
-        graph.replay()
-        return out
+            entry.graph = graph
+        entry.graph.replay()
+        return entry.out
+
+    @torch.no_grad()
+    def forward_graphed(self, points, offsets):
+        """forward_device + pack replayed from a CUDA graph.
+
+        Every stage has static shapes and device-resident counts, and the voxelizer reads the cloud offsets from a
+        device tensor, so the whole forward -- ~50 det3d_b200 launches plus the torch glue -- is one graph launch, and
+        one graph per (batch, bucket, ndim) serves clouds of any size: `bucket` (bucket_of) is the point capacity of the
+        graph's static input buffer.  `offsets` is a host list [0, n0, n0+n1, ...] (ValueError if malformed); it is
+        copied to the device only when it differs from the graph's previous replay.  `points` [offsets[-1], ndim] may
+        live on the host (pinned) or the device; it is copied into the graph's static input buffer.
+        Returns the packed detections [B, D, nd+3] (a static buffer: consume before the next call)."""
+        offsets = self.check_offsets(offsets, points.shape[0])
+        entry = self._graph_entry(len(offsets) - 1, offsets[-1], points.shape[1])
+        entry.points[:offsets[-1]].copy_(points, non_blocking=True)
+        return self._replay(entry, offsets)
 
     @staticmethod
     def pack(det):
@@ -145,18 +184,29 @@ class InferencePipeline:
                           det["valid"].float().unsqueeze(-1)], dim=-1).contiguous()
 
     @torch.no_grad()
-    def infer_host(self, clouds, pinned_out=None):
+    def infer_host(self, clouds, pinned_out=None, graphed=False):
         """clouds: list of pinned (or plain) host float32 tensors [N_i, ndim].
-        H2D copy, forward, D2H of the packed detections.  Returns a host tensor [B, D, nd+3]."""
+        H2D copy, forward, D2H of the packed detections.  Returns a host tensor [B, D, nd+3].
+        graphed=True copies the clouds into the static input of the (batch, bucket) graph and replays it
+        (forward_graphed); the detections are the same bits."""
         offsets = [0]
         for c in clouds:
             offsets.append(offsets[-1] + c.shape[0])
         ndim = clouds[0].shape[1]
-        pts = torch.empty((offsets[-1], ndim), dtype=torch.float32, device=self.device)
-        for c, a, b in zip(clouds, offsets[:-1], offsets[1:]):
-            pts[a:b].copy_(c, non_blocking=True)
+        if graphed:
+            self.check_offsets(offsets)
+        else:
+            pts = torch.empty((offsets[-1], ndim), dtype=torch.float32, device=self.device)
+            for c, a, b in zip(clouds, offsets[:-1], offsets[1:]):
+                pts[a:b].copy_(c, non_blocking=True)
         for _attempt in range(2):
-            packed = self.pack(self.forward_device(pts, offsets))
+            if graphed:         # (a re-run after an overflow captures a new graph: check_overflow dropped them all)
+                entry = self._graph_entry(len(clouds), offsets[-1], ndim)
+                for c, a, b in zip(clouds, offsets[:-1], offsets[1:]):
+                    entry.points[a:b].copy_(c, non_blocking=True)
+                packed = self._replay(entry, offsets)
+            else:
+                packed = self.pack(self.forward_device(pts, offsets))
             if pinned_out is None:
                 pinned_out = torch.empty(packed.shape, dtype=torch.float32, pin_memory=True)
             pinned_out.copy_(packed, non_blocking=True)
@@ -178,3 +228,17 @@ class InferencePipeline:
             m = row[:, -1] > 0.5
             out.append(dict(box3d_lidar=row[m, :-3], scores=row[m, -3], label_preds=row[m, -2].long()))
         return out
+
+
+class _GraphEntry:
+    """Static buffers of one captured forward: points [bucket, ndim], device offsets [batch + 1] and their pinned
+    staging copy, the graph and its packed output."""
+
+    def __init__(self, bucket, batch, ndim, device):
+        self.points = torch.zeros((bucket, ndim), dtype=torch.float32, device=device)
+        self.offsets = torch.zeros(batch + 1, dtype=torch.int32, device=device)
+        self.staging = torch.zeros(batch + 1, dtype=torch.int32, pin_memory=True)
+        self.copied = torch.cuda.Event()
+        self.last_offsets = None
+        self.graph = None
+        self.out = None

@@ -26,6 +26,12 @@ class Voxelizer:
       voxels [cap, max_points, ndim] (optional), coors [cap, 4] (b,z,y,x),
       num_points [cap], mean [cap, ndim], counts int32[batch+1] (last = total rows).
     Only the first counts[-1] rows are defined.
+
+    `offsets` may instead be an int32 cuda tensor [batch+1] (d3b_voxelize_dev): then points.shape[0] is a capacity,
+    rows at or past offsets[-1] are never read, and nothing the host passes depends on the cloud sizes, so the call can
+    be captured in a CUDA graph and replayed for clouds of any size.  out["status"] (int32[1]) is then 1 if the offsets
+    were not 0 = off[0] <= ... <= off[batch] <= capacity (the call ran on them clamped into that shape), else 0.
+    The results are bit-identical to the host-offsets call on the same clouds.
     """
 
     def __init__(self, voxel_size, point_cloud_range, max_num_points, max_voxels, want_voxels=True,
@@ -50,8 +56,9 @@ class Voxelizer:
         cfg.max_voxels = self.max_voxels
         return cfg
 
-    def _buffers(self, n_total, batch, ndim, device):
-        key = (batch, ndim, device)
+    def _buffers(self, n_total, batch, ndim, device, fixed_capacity=False):
+        # With device offsets the buffers of each capacity are kept for good: a captured graph holds their addresses
+        key = (batch, ndim, device, n_total) if fixed_capacity else (batch, ndim, device)
         b = self._bufs.get(key)
         if b is not None and b["n_cap"] >= n_total:
             return b
@@ -66,6 +73,7 @@ class Voxelizer:
             "coors": torch.empty((cap, 4), dtype=torch.int32, device=device),
             "num_points": torch.empty(cap, dtype=torch.int32, device=device),
             "counts": torch.zeros(batch + 1, dtype=torch.int32, device=device),
+            "status": torch.zeros(1, dtype=torch.int32, device=device),
             "voxels": torch.empty((cap, self.max_num_points, ndim), dtype=torch.float32, device=device)
             if self.want_voxels else None,
             "mean": torch.empty((cap, ndim), dtype=torch.float32, device=device) if self.want_mean else None,
@@ -76,23 +84,38 @@ class Voxelizer:
     def __call__(self, points, offsets=None):
         assert points.is_cuda and points.dtype == torch.float32 and points.dim() == 2
         points = points.contiguous()
-        n_total, ndim = points.shape
+        n_rows, ndim = points.shape
         if offsets is None:
-            offsets = [0, n_total]
+            offsets = [0, n_rows]
+        on_device = torch.is_tensor(offsets) and offsets.is_cuda
+        if on_device:
+            if offsets.dtype != torch.int32 or offsets.dim() != 1 or offsets.device != points.device:
+                raise ValueError("device offsets must be an int32 vector on the points' device")
+            offsets = offsets.contiguous()
         batch = len(offsets) - 1
-        b = self._buffers(n_total, batch, ndim, points.device)
-        off = (C.c_int32 * (batch + 1))(*[int(o) for o in offsets])
-        with _lib.on_device_of(points), _lib.timed("voxelize", n_points=n_total, ndim=ndim, batch=batch):
-            st = _lib.lib().d3b_voxelize(
-                C.byref(b["cfg"]), points.data_ptr() if n_total > 0 else None, off, batch,
-                _lib.ptr(b["voxels"]), b["coors"].data_ptr(), b["num_points"].data_ptr(), _lib.ptr(b["mean"]),
-                b["counts"].data_ptr(), b["ws"].data_ptr(), b["ws"].numel(), _lib.current_stream(),
-            )
-        _lib.check(st, "d3b_voxelize")
+        b = self._buffers(n_rows, batch, ndim, points.device, fixed_capacity=on_device)
+        with _lib.on_device_of(points), _lib.timed("voxelize", n_points=n_rows, ndim=ndim, batch=batch):
+            if on_device:
+                st = _lib.lib().d3b_voxelize_dev(
+                    C.byref(b["cfg"]), points.data_ptr() if n_rows > 0 else None, n_rows, offsets.data_ptr(), batch,
+                    _lib.ptr(b["voxels"]), b["coors"].data_ptr(), b["num_points"].data_ptr(), _lib.ptr(b["mean"]),
+                    b["counts"].data_ptr(), b["status"].data_ptr(), b["ws"].data_ptr(), b["ws"].numel(),
+                    _lib.current_stream(),
+                )
+            else:
+                off = (C.c_int32 * (batch + 1))(*[int(o) for o in offsets])
+                st = _lib.lib().d3b_voxelize(
+                    C.byref(b["cfg"]), points.data_ptr() if n_rows > 0 else None, off, batch,
+                    _lib.ptr(b["voxels"]), b["coors"].data_ptr(), b["num_points"].data_ptr(), _lib.ptr(b["mean"]),
+                    b["counts"].data_ptr(), b["ws"].data_ptr(), b["ws"].numel(), _lib.current_stream(),
+                )
+        _lib.check(st, "d3b_voxelize_dev" if on_device else "d3b_voxelize")
         out = {k: b[k] for k in ("voxels", "coors", "num_points", "mean", "counts")}
+        if on_device:
+            out["status"] = b["status"]
         # the per-voxel point-index lists the voxelizer built on the way ([batch][max_voxels][max_points] indices into
         # `points`, valid until the next call): what the fused pillar reader consumes instead of `voxels`
         out["point_lists"] = dict(points=points, lists_ptr=_lib.lib().d3b_voxelize_point_lists(
-            C.byref(b["cfg"]), n_total, batch, b["ws"].data_ptr()), batch=batch, max_voxels=self.max_voxels,
+            C.byref(b["cfg"]), n_rows, batch, b["ws"].data_ptr()), batch=batch, max_voxels=self.max_voxels,
             max_points=self.max_num_points, keepalive=b["ws"])
         return out

@@ -81,6 +81,18 @@ int d3b_voxelize(const d3b_voxel_cfg* cfg, const float* points, const int32_t* c
                  float* mean_feats, int32_t* voxel_counts, void* workspace,
                  size_t workspace_bytes, void* stream);
 
+/* d3b_voxelize with the cloud offsets in DEVICE memory, for graph replay over clouds of any size.
+ * points            [point_capacity, ndim] f32 device; rows at or past off[batch] are never read
+ * cloud_offsets_dev [batch + 1] i32 DEVICE
+ * status            [1] i32 device or NULL: set to 1 if the offsets were not 0 = off[0] <= ... <= off[batch] <= point_capacity;
+ *                   they are then clamped into that shape before any point index is formed (0 when they were)
+ * workspace: d3b_voxelize_workspace_bytes(cfg, point_capacity, batch); point lists: d3b_voxelize_point_lists(cfg, point_capacity, batch, ws)
+ * Outputs are bit-identical to d3b_voxelize's on the same clouds, for any capacity >= off[batch]. */
+int d3b_voxelize_dev(const d3b_voxel_cfg* cfg, const float* points, int32_t point_capacity,
+                     const int32_t* cloud_offsets_dev, int32_t batch, float* voxels, int32_t* coors,
+                     int32_t* num_points, float* mean_feats, int32_t* voxel_counts, int32_t* status,
+                     void* workspace, size_t workspace_bytes, void* stream);
+
 /* Multi-sweep ingest (nuScenes): raw sweeps of one sample -> one cloud [n, n_feat + 1] = (x, y, z, .., time lag).
  * replaces read_file / remove_close / read_sweep and the NuScenes branch of LoadPointCloudFromFile.__call__,
  * det3d/datasets/pipelines/loading.py:17-64,98-124.

@@ -8,6 +8,8 @@ the whole hot path on its shard, ONE all-gather of the fixed-shape detections ov
 
 --check: rank 0 also runs ALL clouds by itself (same per-call batch size) and asserts that the gathered detections are
 bit-identical to the single-rank result -- BASELINE configs[3] (CBGS, 35k points, 32 clouds over 8 GPUs) at its stated size.
+--graphed: every batch replays the CUDA graph of its (batch, point-capacity bucket) (infer_host(graphed=True)).
+--variable-sizes: per-cloud point counts drawn uniformly from [0.6 N, N] (seeded), as real frames have.
 """
 import argparse
 import json
@@ -25,6 +27,8 @@ def main():
     ap.add_argument("--config", default="cbgs", choices=["second", "pillars", "cbgs"])
     ap.add_argument("--clouds", type=int, default=32)
     ap.add_argument("--check", action="store_true")
+    ap.add_argument("--graphed", action="store_true", help="replay one CUDA graph per (batch, point-capacity bucket)")
+    ap.add_argument("--variable-sizes", action="store_true", help="per-cloud point counts uniform in [0.6 N, N] (seeded)")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     import torch
@@ -42,12 +46,17 @@ def main():
     assert a.clouds % world == 0, "--clouds must be a multiple of the world size"
     b_local = a.clouds // world
     clouds = bench.make_clouds(args, a.clouds, 4242, cfg.voxel_generator.range)      # same clouds on every rank
+    if a.variable_sizes:
+        import numpy as np
+        n = args.wl["n_points"]
+        sizes = np.random.default_rng(4243).integers(int(0.6 * n), n + 1, a.clouds)
+        clouds = [c[:k] for c, k in zip(clouds, sizes)]
 
     def run(indices):
         out = []
         for i0 in range(0, len(indices), b_local):
             chunk = [torch.from_numpy(clouds[i]) for i in indices[i0:i0 + b_local]]
-            out.append(pipe.infer_host(chunk).clone())
+            out.append(pipe.infer_host(chunk, graphed=a.graphed).clone())
         return torch.cat(out)
 
     torch.cuda.synchronize()
@@ -58,6 +67,7 @@ def main():
     torch.cuda.synchronize()
     dt = time.perf_counter() - t0
     result = {"config": a.config, "clouds": a.clouds, "world": world, "clouds_per_rank": b_local, "seconds": dt,
+              "graphed": a.graphed, "variable_sizes": a.variable_sizes, "graphs_captured": len(pipe._graphs),
               "detections_per_cloud": [int((ordered[i, :, -1] > 0.5).sum()) for i in range(a.clouds)]}
     ok = True
     if a.check and rank == 0:
