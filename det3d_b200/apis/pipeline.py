@@ -18,6 +18,8 @@ import torch
 
 from det3d_b200 import _lib
 from det3d_b200.core.anchor.anchor_generator import anchors_for_tasks
+from det3d_b200.datasets.pipelines.loading import (BatchedIngest, check_sweep_samples, ingest_sweeps_batched,
+                                                    stage_raw_sweeps, sweep_table_capacity)
 from det3d_b200.models import build_detector
 from det3d_b200.ops.point_cloud.voxelize import Voxelizer
 
@@ -46,7 +48,9 @@ class InferencePipeline:
         self._anchors = [torch.from_numpy(a).to(self.device) for a in anchors]
         self._anchor_cache = {}
         self.strict_fp32 = strict_fp32
-        self._graphs = collections.OrderedDict()      # (batch, bucket, ndim) -> _GraphEntry, least recently used first
+        # (batch, bucket, ndim) -> _GraphEntry and (batch, raw bucket, table capacity, raw_stride, n_feat) ->
+        # _SweepGraphEntry (infer_sweeps), least recently used first
+        self._graphs = collections.OrderedDict()
         self.max_graphs = 8
         self._ovf_host = None
 
@@ -143,17 +147,21 @@ class InferencePipeline:
             entry.offsets.copy_(entry.staging, non_blocking=True)
             entry.copied.record()
             entry.last_offsets = key
+        return self._run_graph(entry, lambda: self.pack(self.forward_device(entry.points, entry.offsets)))
+
+    def _run_graph(self, entry, step):
+        """Capture `step` (which returns the packed detections) into entry.graph on first use, then replay it."""
         if entry.graph is None:
             side = torch.cuda.Stream(device=self.device)
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
                 for _ in range(3):                      # warm-up: lazy buffers, weight packing, cuDNN plans
-                    self.pack(self.forward_device(entry.points, entry.offsets))
+                    step()
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                entry.out = self.pack(self.forward_device(entry.points, entry.offsets))
+                entry.out = step()
                 _lib.graph_mark("end")          # (bench.py's in-graph stage timing; nothing unless _lib.GRAPH_MARKS is set)
             entry.graph = graph
         entry.graph.replay()
@@ -207,18 +215,75 @@ class InferencePipeline:
                 packed = self._replay(entry, offsets)
             else:
                 packed = self.pack(self.forward_device(pts, offsets))
-            if pinned_out is None:
-                pinned_out = torch.empty(packed.shape, dtype=torch.float32, pin_memory=True)
-            pinned_out.copy_(packed, non_blocking=True)
-            flag = self.overflow_flag()
-            if flag is not None:
-                if self._ovf_host is None:
-                    self._ovf_host = torch.zeros(1, dtype=torch.int32, pin_memory=True)
-                self._ovf_host.copy_(flag, non_blocking=True)
-            torch.cuda.current_stream().synchronize()
-            if flag is None or not self.check_overflow(int(self._ovf_host[0])):
+            pinned_out, rerun = self._fetch(packed, pinned_out)
+            if not rerun:
                 break
         return pinned_out
+
+    def _fetch(self, packed, pinned_out):
+        """D2H of the packed detections and of the f16-range flag, then one sync.  Returns (pinned_out, rerun): rerun is
+        True when the flag was raised and the model has switched to tf32x3 (check_overflow)."""
+        if pinned_out is None:
+            pinned_out = torch.empty(packed.shape, dtype=torch.float32, pin_memory=True)
+        pinned_out.copy_(packed, non_blocking=True)
+        flag = self.overflow_flag()
+        if flag is not None:
+            if self._ovf_host is None:
+                self._ovf_host = torch.zeros(1, dtype=torch.int32, pin_memory=True)
+            self._ovf_host.copy_(flag, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        return pinned_out, flag is not None and self.check_overflow(int(self._ovf_host[0]))
+
+    @torch.no_grad()
+    def infer_sweeps(self, samples, pinned_out=None, graphed=False, n_feat=4, radius=1.0):
+        """Multi-sweep samples -> host detections [B, D, nd+3], as infer_host.
+
+        samples: [(raw_sweeps, transforms, time_lags), ...], one per cloud, each with ingest_sweeps' contract (raw
+        float32 [n, raw_stride] host arrays or pinned tensors, key frame first and neither filtered nor transformed
+        unless given a transform; 4x4 or None transforms; one time lag per sweep).  One batched ingest
+        (d3b_ingest_sweeps_dev) writes the clouds and their device offsets, which the voxelizer reads directly: no host
+        sync before the D2H of the detections.  graphed=True replays one CUDA graph covering ingest, voxelize and
+        forward per (B, raw bucket, sweep-table capacity, raw_stride, n_feat) (bucket_of of the raw total); the raw
+        sweeps are copied into its static raw buffer and the sweep table is copied H2D only when it changed.  Raises
+        ValueError before anything is enqueued when the samples are malformed or n_feat + 1 is not the reader's
+        feature count.  The overflow fallback is infer_host's."""
+        if n_feat + 1 != self.num_point_features:
+            raise ValueError("ingested clouds have n_feat + 1 = %d features, the reader takes %d"
+                             % (n_feat + 1, self.num_point_features))
+        samples = list(samples)
+        stride, sizes = check_sweep_samples(samples, n_feat)
+        batch, total = len(samples), sum(map(sum, sizes))
+        bucket = self.bucket_of(total)
+        table_cap = sweep_table_capacity(sum(map(len, sizes)), batch)
+        if not graphed:
+            # the voxelizer keeps its device-offset buffers per capacity: the bucket bounds how many it keeps
+            points, cloud_offsets = ingest_sweeps_batched(samples, radius, n_feat, self.device, capacity=bucket)
+        for _attempt in range(2):
+            if graphed:         # (a re-run after an overflow captures a new graph: check_overflow dropped them all)
+                entry = self._sweep_graph_entry(batch, bucket, table_cap, stride, n_feat, radius)
+                entry.stage(samples, sizes)
+                ing = entry.ingest
+                packed = self._run_graph(entry, lambda: self.pack(self.forward_device(*ing.launch())))
+            else:
+                packed = self.pack(self.forward_device(points, cloud_offsets))
+            pinned_out, rerun = self._fetch(packed, pinned_out)
+            if not rerun:
+                break
+        return pinned_out
+
+    def _sweep_graph_entry(self, batch, bucket, table_cap, raw_stride, n_feat, radius):
+        """The infer_sweeps graph of (batch, bucket, table_cap, raw_stride, n_feat), in the LRU of forward_graphed."""
+        key = (batch, bucket, table_cap, raw_stride, n_feat)
+        entry = self._graphs.get(key)
+        if entry is not None and entry.ingest.radius == radius:
+            self._graphs.move_to_end(key)
+            return entry
+        self._graphs.pop(key, None)
+        while len(self._graphs) >= self.max_graphs:
+            self._graphs.popitem(last=False)
+        entry = self._graphs[key] = _SweepGraphEntry(BatchedIngest(batch, bucket, table_cap, raw_stride, n_feat, radius,
+                                                                   self.device))
+        return entry
 
     @staticmethod
     def unpack(packed_host):
@@ -242,3 +307,31 @@ class _GraphEntry:
         self.last_offsets = None
         self.graph = None
         self.out = None
+
+
+class _SweepGraphEntry:
+    """Static buffers of one captured infer_sweeps forward: the BatchedIngest (raw sweeps, sweep table, clouds, cloud
+    offsets), the pinned staging of the table and of raw sweeps that are not pinned already, the graph and its output."""
+
+    def __init__(self, ingest):
+        self.ingest = ingest
+        self.table_staging = torch.zeros(ingest.table.numel(), dtype=torch.uint8, pin_memory=True)
+        self.raw_staging = None
+        self.copied = torch.cuda.Event()
+        self.last_table = None
+        self.graph = None
+        self.out = None
+
+    def stage(self, samples, sizes):
+        """Enqueue the H2D copies of the raw sweeps and, when it differs from the previous replay's, of the table."""
+        # the pinned staging buffers may still feed the previous copies: wait for those before rewriting them
+        self.copied.synchronize()
+        table = self.ingest.host_table(samples, sizes)
+        if self.last_table is None or not np.array_equal(table, self.last_table):
+            self.table_staging.numpy()[:] = table
+            self.ingest.table.copy_(self.table_staging, non_blocking=True)
+            self.last_table = table
+        if self.raw_staging is None and not all(torch.is_tensor(r) and r.is_pinned() for s in samples for r in s[0]):
+            self.raw_staging = torch.empty(self.ingest.raw.shape, dtype=torch.float32, pin_memory=True)
+        stage_raw_sweeps(samples, sizes, self.ingest.raw, self.raw_staging)
+        self.copied.record()

@@ -8,6 +8,10 @@ the 1 m `remove_close` filter of the sweeps (:34-43), the float64 rigid transfor
 the concatenation (:115-124) -- is one call over the raw bytes of all sweeps.  `res["lidar"]` receives the same
 numpy fields as the reference (`points`, `times`, `combined`) plus `combined_cuda`, the device tensor the
 voxelizer consumes directly (no second H2D copy).
+
+`ingest_sweeps_batched` does the same for a batch of samples in one d3b_ingest_sweeps_dev call: the sweep table lives
+in device memory and the per-sample cloud offsets stay there, in the form the voxelizer's device-offset path takes, so
+nothing between the raw sweeps and the detections waits on the host (InferencePipeline.infer_sweeps).
 """
 import ctypes as C
 from pathlib import Path
@@ -72,6 +76,183 @@ def ingest_sweeps(raw_sweeps, transforms, time_lags, radius=1.0, n_feat=4, devic
         _lib.check(st, "d3b_ingest_sweeps")
         n = int(n_out.item())            # API boundary: the reference returns exactly-sized arrays
     return out[:n]
+
+
+MAX_SWEEPS = 16          # D3B_INGEST_MAX_SWEEPS: sweeps per sample, key frame included
+MAX_BATCH = 64           # samples per batched ingest, as the voxelizer's batch
+
+
+def check_sweep_samples(samples, n_feat=4):
+    """Host-side validation of a batch of multi-sweep samples [(raw_sweeps, transforms, time_lags), ...] with
+    ingest_sweeps' per-sample contract: raises ValueError, before anything is enqueued.  Raw sweeps are float32
+    [n, raw_stride] numpy arrays or CPU tensors (pinned ones are copied to the device directly), one raw_stride for the
+    whole batch.  Returns (raw_stride, per-sample lists of sweep sizes)."""
+    samples = list(samples)
+    if not 1 <= len(samples) <= MAX_BATCH:
+        raise ValueError("a batch holds 1 to %d samples, got %d" % (MAX_BATCH, len(samples)))
+    if n_feat < 3:
+        raise ValueError("n_feat must be >= 3, got %d" % n_feat)
+    stride, sizes = None, []
+    for b, sample in enumerate(samples):
+        if len(sample) != 3:
+            raise ValueError("sample %d: expected (raw_sweeps, transforms, time_lags)" % b)
+        raws, tms, lags = sample
+        if not 1 <= len(raws) <= MAX_SWEEPS:
+            raise ValueError("sample %d: %d sweeps, expected 1 to %d (key frame included)" % (b, len(raws), MAX_SWEEPS))
+        if len(tms) != len(raws) or len(lags) != len(raws):
+            raise ValueError("sample %d: %d sweeps but %d transforms and %d time lags" % (b, len(raws), len(tms), len(lags)))
+        for s, r in enumerate(raws):
+            if torch.is_tensor(r):
+                ok = r.dtype == torch.float32 and r.device.type == "cpu"
+            else:
+                ok = isinstance(r, np.ndarray) and r.dtype == np.float32
+            if not ok or r.ndim != 2:
+                raise ValueError("sample %d sweep %d: raw points must be a 2-D float32 host array" % (b, s))
+            stride = int(r.shape[1]) if stride is None else stride
+            if int(r.shape[1]) != stride:
+                raise ValueError("sample %d sweep %d: raw stride %d, the batch has %d" % (b, s, r.shape[1], stride))
+        for s, t in enumerate(tms):
+            if t is not None and np.shape(t) != (4, 4):
+                raise ValueError("sample %d sweep %d: transform must be 4x4 or None, got shape %s" % (b, s, np.shape(t)))
+        if np.asarray(lags, dtype=np.float64).shape != (len(raws),):
+            raise ValueError("sample %d: time lags must be %d numbers" % (b, len(raws)))
+        sizes.append([int(r.shape[0]) for r in raws])
+    if stride < n_feat:
+        raise ValueError("raw_stride %d < n_feat %d" % (stride, n_feat))
+    if sum(map(sum, sizes)) > 1 << 30:
+        raise ValueError("more than 2^30 raw points in one batch")
+    return stride, sizes
+
+
+def sweep_table_capacity(n_sweeps, batch):
+    """Sweep capacity of a batched ingest's device table: the smallest power of two >= n_sweeps, at most 16 * batch."""
+    return min(1 << (max(int(n_sweeps), 1) - 1).bit_length(), MAX_SWEEPS * batch)
+
+
+def sweep_table_views(buf, sweep_capacity, batch):
+    """Typed views over one byte buffer (numpy or torch) holding a device sweep table, laid out as
+    transforms f64 [S, 16] | sweep_offsets i32 [S + 1] | sample_sweeps i32 [B + 1] | time_lag f32 [S] | flags u8 [S]."""
+    S, B = sweep_capacity, batch
+    parts, views, at = (("transforms", 8, S * 16), ("sweep_offsets", 4, S + 1), ("sample_sweeps", 4, B + 1),
+                        ("time_lag", 4, S), ("flags", 1, S)), {}, 0
+    is_np = isinstance(buf, np.ndarray)
+    for name, size, count in parts:
+        raw = buf[at:at + size * count]
+        dt = {8: np.float64, 4: np.float32 if name == "time_lag" else np.int32, 1: np.uint8}[size]
+        views[name] = raw.view(dt) if is_np else raw.view(_TORCH_DTYPE[dt])
+        at += size * count
+    return views
+
+
+_TORCH_DTYPE = {np.float64: torch.float64, np.float32: torch.float32, np.int32: torch.int32, np.uint8: torch.uint8}
+
+
+def sweep_table_bytes(sweep_capacity, batch):
+    return sweep_capacity * (16 * 8 + 4 + 4 + 1) + 4 * (batch + 2)
+
+
+def fill_sweep_table(views, samples, sizes):
+    """Writes the table of `samples` (validated by check_sweep_samples) into host views (sweep_table_views).  As
+    ingest_sweeps: the key frame (sweep 0 of each sample) is never filtered, its transform and lag are used as given."""
+    for v in views.values():
+        v[:] = 0
+    s = 0
+    rows = 0
+    views["sweep_offsets"][0] = 0
+    views["sample_sweeps"][0] = 0
+    for b, ((_raws, tms, lags), n) in enumerate(zip(samples, sizes)):
+        lags = np.asarray(lags, np.float64).astype(np.float32)         # times.astype(points.dtype), loading.py:119
+        for j, t in enumerate(tms):
+            if t is not None:
+                views["transforms"][s * 16:(s + 1) * 16] = np.asarray(t, np.float64).reshape(16)
+            views["flags"][s] = (1 if t is not None else 0) | (2 if j > 0 else 0)
+            views["time_lag"][s] = lags[j]
+            rows += n[j]
+            views["sweep_offsets"][s + 1] = rows
+            s += 1
+        views["sample_sweeps"][b + 1] = s
+    views["sweep_offsets"][s + 1:] = rows         # unused table rows: empty sweeps past the last sample
+
+
+def stage_raw_sweeps(samples, sizes, raw_dev, staging=None):
+    """Enqueues the H2D copies of every raw sweep into raw_dev, back to back in sample order.  Pinned tensors are copied
+    directly; anything else goes through the pinned `staging` buffer ([>= total, raw_stride], allocated when None)."""
+    at = 0
+    for (raws, _tms, _lags), n in zip(samples, sizes):
+        for r, k in zip(raws, n):
+            if k:
+                src = r if torch.is_tensor(r) and r.is_pinned() else None
+                if src is None:
+                    if staging is None:
+                        staging = torch.empty(raw_dev.shape, dtype=torch.float32, pin_memory=True)
+                    src = staging[at:at + k]
+                    src.copy_(torch.as_tensor(r))
+                raw_dev[at:at + k].copy_(src, non_blocking=True)
+            at += k
+    return at
+
+
+class BatchedIngest:
+    """Device buffers of one batched-ingest shape -- raw [raw_capacity, raw_stride], the sweep table, the ingested
+    clouds [raw_capacity, n_feat + 1], cloud_offsets [B + 1], status, workspace -- and the d3b_ingest_sweeps_dev call
+    over them.  The addresses never change, so a captured CUDA graph can hold them."""
+
+    def __init__(self, batch, raw_capacity, sweep_capacity, raw_stride, n_feat=4, radius=1.0, device="cuda"):
+        dev = torch.device(device)
+        self.batch, self.raw_capacity, self.sweep_capacity = batch, raw_capacity, sweep_capacity
+        self.raw_stride, self.n_feat, self.radius = raw_stride, n_feat, radius
+        self.raw = torch.empty((raw_capacity, raw_stride), dtype=torch.float32, device=dev)   # rows past the live total are never read
+        self.table = torch.zeros(sweep_table_bytes(sweep_capacity, batch), dtype=torch.uint8, device=dev)
+        self.tables = sweep_table_views(self.table, sweep_capacity, batch)
+        self.out = torch.empty((raw_capacity, n_feat + 1), dtype=torch.float32, device=dev)
+        self.cloud_offsets = torch.zeros(batch + 1, dtype=torch.int32, device=dev)
+        self.status = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.ws = torch.empty(_lib.lib().d3b_ingest_dev_workspace_bytes(raw_capacity, sweep_capacity), dtype=torch.uint8,
+                              device=dev)
+
+    def host_table(self, samples, sizes, out=None):
+        """The table image of `samples` as uint8 host bytes (into `out`, e.g. a pinned buffer, when given)."""
+        buf = np.zeros(self.table.numel(), np.uint8) if out is None else out
+        fill_sweep_table(sweep_table_views(buf, self.sweep_capacity, self.batch), samples, sizes)
+        return buf
+
+    def launch(self):
+        """Ingests the raw sweeps under the device table into out / cloud_offsets (three kernels, no host sync)."""
+        t = self.tables
+        with _lib.on_device_of(self.raw), _lib.timed("ingest_sweeps", batch=self.batch, capacity=self.raw_capacity):
+            st = _lib.lib().d3b_ingest_sweeps_dev(
+                self.raw.data_ptr(), self.raw_capacity, self.raw_stride, self.n_feat, t["sweep_offsets"].data_ptr(),
+                t["sample_sweeps"].data_ptr(), t["transforms"].data_ptr(), t["time_lag"].data_ptr(),
+                t["flags"].data_ptr(), self.sweep_capacity, self.batch, C.c_float(self.radius), self.out.data_ptr(),
+                self.cloud_offsets.data_ptr(), self.status.data_ptr(), self.ws.data_ptr(), self.ws.numel(),
+                _lib.current_stream())
+        _lib.check(st, "d3b_ingest_sweeps_dev")
+        return self.out, self.cloud_offsets
+
+
+def ingest_sweeps_batched(samples, radius=1.0, n_feat=4, device="cuda", capacity=None, return_ingest=False):
+    """Batched ingest_sweeps: samples = [(raw_sweeps, transforms, time_lags), ...], each with ingest_sweeps' contract
+    (key frame first; it is neither filtered nor transformed unless a transform is given).  One d3b_ingest_sweeps_dev
+    call, no host sync.  Returns (points [capacity, n_feat + 1], cloud_offsets int32 [B + 1]), both on the device:
+    sample b's cloud is points[cloud_offsets[b]:cloud_offsets[b + 1]], bit-identical to ingest_sweeps on that sample;
+    rows past cloud_offsets[B] are undefined.  capacity (default: the raw total) must be >= the raw total."""
+    if not torch.cuda.is_available():
+        raise RuntimeError("det3d_b200: the multi-sweep ingest needs a CUDA device (there is no CPU fallback)")
+    samples = list(samples)
+    stride, sizes = check_sweep_samples(samples, n_feat)
+    total = sum(map(sum, sizes))
+    capacity = max(total, 1) if capacity is None else int(capacity)
+    if capacity < total:
+        raise ValueError("capacity %d < %d raw points" % (capacity, total))
+    ing = BatchedIngest(len(samples), capacity, sweep_table_capacity(sum(map(len, sizes)), len(samples)), stride,
+                        n_feat, radius, device)
+    table = torch.empty(ing.table.numel(), dtype=torch.uint8, pin_memory=True)
+    ing.host_table(samples, sizes, out=table.numpy())
+    with torch.cuda.device(ing.raw.device):
+        ing.table.copy_(table, non_blocking=True)
+        stage_raw_sweeps(samples, sizes, ing.raw)
+        points, offsets = ing.launch()
+    return (points, offsets, ing) if return_ingest else (points, offsets)
 
 
 @PIPELINES.register_module

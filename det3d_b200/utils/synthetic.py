@@ -49,6 +49,32 @@ def lidar_like_cloud(n, point_cloud_range, ndim=4, seed=0):
     return np.ascontiguousarray(pts[:n])
 
 
+def lidar_like_sweeps(sizes, point_cloud_range, seed=0, raw_stride=5, max_yaw=0.1, max_shift=5.0, lag_step=0.05,
+                      close_fraction=0.0):
+    """One nuScenes-style multi-sweep sample: (raw_sweeps, transforms, time_lags) for ingest_sweeps.  Sweep s is a seeded
+    lidar_like_cloud of sizes[s] raw records (raw_stride floats), the key frame (s = 0) untransformed, every other
+    sweep under a seeded rigid motion (yaw <= max_yaw rad, translation <= max_shift m) with lag lag_step * s.
+    close_fraction of each sweep's points are moved inside the 1 m remove_close box."""
+    rng = np.random.default_rng(seed)
+    raws, tms, lags = [], [], []
+    for s, n in enumerate(sizes):
+        p = lidar_like_cloud(int(n), point_cloud_range, raw_stride, seed * 1000 + s) if n else np.zeros((0, raw_stride), np.float32)
+        k = int(round(close_fraction * p.shape[0]))
+        if k:
+            p[:k, :2] = rng.uniform(-0.99, 0.99, (k, 2)).astype(np.float32)
+        raws.append(p)
+        if s == 0:
+            tms.append(None)
+        else:
+            a = rng.uniform(-max_yaw, max_yaw)
+            t = np.eye(4)
+            t[:2, :2] = [[np.cos(a), -np.sin(a)], [np.sin(a), np.cos(a)]]
+            t[:3, 3] = rng.uniform(-1, 1, 3) * (max_shift / np.sqrt(3))
+            tms.append(t)
+        lags.append(lag_step * s)
+    return raws, tms, lags
+
+
 def nms_boxes_xyxyr(n, seed=0, clustered=False, extent=100.0):
     """[n,5] x1,y1,x2,y2,ry + distinct scores (SURVEY 8d C5)."""
     rng = np.random.default_rng(seed)

@@ -109,6 +109,30 @@ int d3b_ingest_sweeps(const float* raw, const int32_t* sweep_offsets, int32_t n_
                       const uint8_t* filter_close, float radius, float* out, int32_t out_cap, int32_t* n_out,
                       void* workspace, size_t workspace_bytes, void* stream);
 
+/* d3b_ingest_sweeps for a batch of samples with the sweep table in DEVICE memory, for graph replay over sweeps of any
+ * size; runs the same three kernels, whatever the batch (no host sync).  S = sweep_capacity, 1 <= batch <= 64,
+ * 1 <= S <= D3B_INGEST_MAX_SWEEPS * batch.
+ * raw            [raw_capacity, raw_stride] f32 device: every sweep of every sample back to back, each sample's key frame
+ *                first; rows at or past sweep_offsets[sample_sweeps[batch]] are never read
+ * sweep_offsets  [S + 1] i32 DEVICE, raw rows: sweep s owns rows [sweep_offsets[s], sweep_offsets[s + 1])
+ * sample_sweeps  [batch + 1] i32 DEVICE: sample b owns sweeps [sample_sweeps[b], sample_sweeps[b + 1])
+ * transforms     [S, 16] f64 DEVICE row-major 4x4, time_lag [S] f32 DEVICE
+ * flags          [S] u8 DEVICE: bit 0 = has_transform, bit 1 = filter_close (as d3b_ingest_sweeps; a key frame has neither)
+ * out            [raw_capacity, n_feat + 1] f32 device: the samples' clouds back to back, each in input order
+ * cloud_offsets  [batch + 1] i32 device: sample b's cloud is rows [cloud_offsets[b], cloud_offsets[b + 1]) of `out` --
+ *                the form d3b_voxelize_dev takes
+ * status         [1] i32 device or NULL: set to 1 if the tables were not 0 = sweep_offsets[0] <= ... <= sweep_offsets[S]
+ *                <= raw_capacity and 0 = sample_sweeps[0] <= ... <= sample_sweeps[batch] <= S; they are then clamped
+ *                into that shape as t[i] = min(max(0, t[1..i]), bound) before any point index is formed (0 when they were)
+ * workspace: d3b_ingest_dev_workspace_bytes(raw_capacity, S).  Each sample's rows are bit-identical to d3b_ingest_sweeps's
+ * output for that sample alone. */
+size_t d3b_ingest_dev_workspace_bytes(int32_t raw_capacity, int32_t sweep_capacity);
+int d3b_ingest_sweeps_dev(const float* raw, int32_t raw_capacity, int32_t raw_stride, int32_t n_feat,
+                          const int32_t* sweep_offsets, const int32_t* sample_sweeps, const double* transforms,
+                          const float* time_lag, const uint8_t* flags, int32_t sweep_capacity, int32_t batch,
+                          float radius, float* out, int32_t* cloud_offsets, int32_t* status, void* workspace,
+                          size_t workspace_bytes, void* stream);
+
 /* ========================================================================= *
  * 2. Rulebook (sparse-convolution index maps)
  *    replaces spconv v1.x `get_indice_pairs` as called by SubMConv3d /
