@@ -130,6 +130,8 @@ SIGNATURES = {
     "d3b_ingest_sweeps": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _vp, _i32, _vp, _vp, _sz, _vp]),
     "d3b_ingest_dev_workspace_bytes": (_sz, [_i32, _i32]),
     "d3b_ingest_sweeps_dev": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "d3b_ingest_gather_workspace_bytes": (_sz, [_i32, _i32]),
+    "d3b_ingest_sweeps_gather": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _sz, _vp]),
     "d3b_rulebook_workspace_bytes": (_sz, [_i64]),
     "d3b_index_build_hash": (C.c_int, [_vp, _vp, _i32, C.POINTER(SiteIndex), _vp]),
     "d3b_rulebook_subm": (C.c_int, [_vp, _vp, _i32, C.POINTER(SiteIndex), _I3, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -11,6 +11,7 @@ batch index and the VoxelFeatureExtractorV3 mean fused in, anchors are generated
 and cached on the device, and detections come back as fixed-shape tensors.
 """
 import collections
+import numbers
 import warnings
 
 import numpy as np
@@ -18,8 +19,9 @@ import torch
 
 from det3d_b200 import _lib
 from det3d_b200.core.anchor.anchor_generator import anchors_for_tasks
-from det3d_b200.datasets.pipelines.loading import (BatchedIngest, check_sweep_samples, ingest_sweeps_batched,
-                                                    stage_raw_sweeps, sweep_table_capacity)
+from det3d_b200.datasets.pipelines.loading import (MAX_BATCH, MAX_SWEEPS, BatchedIngest, SweepHistory,
+                                                    check_sweep_samples, ingest_sweeps_batched, stage_raw_sweeps,
+                                                    sweep_table_capacity)
 from det3d_b200.models import build_detector
 from det3d_b200.ops.point_cloud.voxelize import Voxelizer
 
@@ -48,8 +50,9 @@ class InferencePipeline:
         self._anchors = [torch.from_numpy(a).to(self.device) for a in anchors]
         self._anchor_cache = {}
         self.strict_fp32 = strict_fp32
-        # (batch, bucket, ndim) -> _GraphEntry and (batch, raw bucket, table capacity, raw_stride, n_feat) ->
-        # _SweepGraphEntry (infer_sweeps), least recently used first
+        # (batch, bucket, ndim) -> _GraphEntry, (batch, raw bucket, table capacity, raw_stride, n_feat) ->
+        # _SweepGraphEntry (infer_sweeps) and ("stream", B, K, slot_capacity, raw_stride, n_feat) -> _StreamGraphEntry
+        # (SweepStream.infer), least recently used first
         self._graphs = collections.OrderedDict()
         self.max_graphs = 8
         self._ovf_host = None
@@ -335,3 +338,173 @@ class _SweepGraphEntry:
             self.raw_staging = torch.empty(self.ingest.raw.shape, dtype=torch.float32, pin_memory=True)
         stage_raw_sweeps(samples, sizes, self.ingest.raw, self.raw_staging)
         self.copied.record()
+
+
+class _StreamGraphEntry:
+    """One captured SweepStream forward: the stream whose buffers the graph holds, the graph and its packed output."""
+
+    def __init__(self, stream):
+        self.stream = stream
+        self.graph = None
+        self.out = None
+
+
+class SweepStream:
+    """B independent LiDAR streams whose sweep histories stay in device memory, feeding infer_sweeps' model.
+
+    Each stream keeps its last K (<= 16) sweeps in slots of one device buffer [B, K, slot_capacity, raw_stride]: push()
+    writes a new sweep into slot (pushes since reset) mod K of its stream with one H2D copy (pinned tensors directly,
+    anything else through a pinned staging buffer), so a sweep is uploaded once however many frames it takes part in.
+    In a frame the newest push of each stream is its key frame (neither filtered nor transformed) and its earlier sweeps
+    follow newest first, each under inv(P_key) @ P_s (float64, on the host) with lag t_key - t_s rounded to float32 and
+    the `radius` remove_close filter, exactly as infer_sweeps treats a sample.  infer() sends only the sweep table (a few
+    KB: offsets, slot starts, transforms, lags, flags) and runs d3b_ingest_sweeps_gather over the slots; the detections
+    are bit-identical to infer_sweeps(samples()).  A stream with fewer than K pushes uses the sweeps it has; reset(b)
+    empties a stream (e.g. at a scene change).
+
+    Not reproduced: the reference draws a sample's sweeps with np.random.choice (a random order, and the voxelizer's
+    output depends on input order); here they are always newest first.  Nor is the reference's nuScenes pose chain: its
+    info files carry a transform_matrix built from ego and calibration poses, which can differ from inv(P_key) @ P_s in
+    the last bits.
+
+    With graphed=True one CUDA graph keyed ("stream", B, K, slot_capacity, raw_stride, n_feat) in the pipeline's LRU
+    covers ingest, voxelize and forward.  Its raw capacity is B * K * slot_capacity, so frames of any size replay it;
+    the slot copies happen outside it.  A graph holds one stream's buffers: a second stream of the same shape on the same
+    pipeline replaces the entry (and recaptures) when it infers."""
+
+    def __init__(self, pipe, batch, history=10, slot_capacity=40000, raw_stride=5, n_feat=4, radius=1.0):
+        if not 1 <= batch <= MAX_BATCH:
+            raise ValueError("batch must be in [1, %d], got %d" % (MAX_BATCH, batch))
+        if not 1 <= history <= MAX_SWEEPS:
+            raise ValueError("history must be in [1, %d] sweeps (key frame included), got %d" % (MAX_SWEEPS, history))
+        if slot_capacity < 1 or batch * history * slot_capacity > 1 << 30:
+            raise ValueError("slot_capacity %d outside [1, 2^30 / (batch * history)]" % slot_capacity)
+        if n_feat < 3 or raw_stride < n_feat:
+            raise ValueError("bad layout: n_feat %d, raw_stride %d" % (n_feat, raw_stride))
+        if n_feat + 1 != pipe.num_point_features:
+            raise ValueError("ingested clouds have n_feat + 1 = %d features, the reader takes %d"
+                             % (n_feat + 1, pipe.num_point_features))
+        self.pipe, self.batch, self.history, self.slot_capacity = pipe, batch, history, slot_capacity
+        self.raw_stride, self.n_feat, self.radius = raw_stride, n_feat, radius
+        self.key = ("stream", batch, history, slot_capacity, raw_stride, n_feat)
+        self.sweeps = SweepHistory(batch, history)
+        self.pending_h2d_bytes = 0                # pushed since the last infer()
+        self.last_h2d_bytes = 0                   # of the last infer(): the pushes before it + its table
+        self._ingest = None                       # device buffers, allocated on the first push
+        self._push_staging = None                 # pinned [B, slot_capacity, raw_stride], allocated on first need
+        self._push_copied = None
+
+    def _buffers(self):
+        """The gather BatchedIngest whose raw buffer holds the slots, and the slots' [B, K, slot_capacity, raw_stride]
+        view of it (allocated on first use)."""
+        if self._ingest is None:
+            B, K = self.batch, self.history
+            self._ingest = BatchedIngest(B, B * K * self.slot_capacity, B * K, self.raw_stride, self.n_feat, self.radius,
+                                         self.pipe.device, gather=True)
+            self._slots = self._ingest.raw.view(B, K, self.slot_capacity, self.raw_stride)
+            self._table_staging = torch.zeros(self._ingest.table.numel(), dtype=torch.uint8, pin_memory=True)
+            self._table_copied = torch.cuda.Event()
+        return self._ingest, self._slots
+
+    def check_push(self, b, raw, pose, timestamp):
+        """Host-side validation of push()'s arguments: raises ValueError.  Returns the number of raw points."""
+        self.sweeps.check_stream(b)
+        if torch.is_tensor(raw):
+            ok = raw.dtype == torch.float32 and raw.device.type == "cpu"
+        else:
+            ok = isinstance(raw, np.ndarray) and raw.dtype == np.float32
+        if not ok or raw.ndim != 2:
+            raise ValueError("stream %d: raw points must be a 2-D float32 host array" % b)
+        if int(raw.shape[1]) != self.raw_stride:
+            raise ValueError("stream %d: raw stride %d, the stream has %d" % (b, raw.shape[1], self.raw_stride))
+        if int(raw.shape[0]) > self.slot_capacity:
+            raise ValueError("stream %d: %d raw points exceed the slot capacity %d" % (b, raw.shape[0], self.slot_capacity))
+        if np.shape(pose) != (4, 4):
+            raise ValueError("stream %d: pose must be a 4x4 matrix, got shape %s" % (b, np.shape(pose)))
+        if not isinstance(timestamp, numbers.Real):
+            raise ValueError("stream %d: timestamp must be a number, got %r" % (b, timestamp))
+        return int(raw.shape[0])
+
+    def push(self, b, raw, pose, timestamp):
+        """Stream b's new sweep, which becomes its key frame: raw float32 [n, raw_stride] host array or tensor (pinned
+        tensors are copied directly and must stay unchanged until the copy has run), pose the sensor-to-world 4x4
+        matrix, timestamp in seconds.  Enqueues one H2D copy into the stream's oldest slot; ValueError before anything
+        is enqueued when an argument is malformed."""
+        rows = self.check_push(b, raw, pose, timestamp)
+        _ing, slots = self._buffers()
+        slot = self.sweeps.next_slot(b)
+        if rows:
+            with torch.cuda.device(slots.device):
+                src = raw if torch.is_tensor(raw) and raw.is_pinned() else None
+                if src is None:
+                    if self._push_staging is None:
+                        self._push_staging = torch.empty((self.batch, self.slot_capacity, self.raw_stride),
+                                                         dtype=torch.float32, pin_memory=True)
+                        self._push_copied = [torch.cuda.Event() for _ in range(self.batch)]
+                    self._push_copied[b].synchronize()          # stream b's staging may still feed its previous copy
+                    src = self._push_staging[b, :rows]
+                    src.copy_(torch.as_tensor(raw))
+                    slots[b, slot, :rows].copy_(src, non_blocking=True)
+                    self._push_copied[b].record()
+                else:
+                    slots[b, slot, :rows].copy_(src, non_blocking=True)
+        self.sweeps.record(b, rows, pose, timestamp)
+        self.pending_h2d_bytes += rows * self.raw_stride * 4
+
+    def reset(self, b):
+        """Forget stream b's history: its next push is a key frame with no earlier sweeps."""
+        self.sweeps.reset(b)
+
+    def samples(self):
+        """The current frame as infer_sweeps' samples [(raw_sweeps, transforms, time_lags), ...], the raw sweeps read
+        back from the device slots: a test oracle and debugging aid (it synchronizes)."""
+        frame = self.sweeps.frame()
+        _ing, slots = self._buffers()
+        return [([slots[b, k, :n].cpu().numpy() for k, n in zip(ks, ns)], tms, lags)
+                for b, (ks, ns, tms, lags) in enumerate(frame)]
+
+    def _stage_table(self):
+        """Writes the current frame's sweep table into the pinned staging buffer and enqueues its H2D copy."""
+        frame = self.sweeps.frame()
+        ing, _slots = self._buffers()
+        K, cap = self.history, self.slot_capacity
+        src = [(b * K + k) * cap for b, (ks, _ns, _tms, _lags) in enumerate(frame) for k in ks]
+        self._table_copied.synchronize()          # the staging buffer may still feed the previous frame's copy
+        ing.host_table([(None, tms, lags) for _ks, _ns, tms, lags in frame], [ns for _ks, ns, _tms, _lags in frame],
+                       out=self._table_staging.numpy(), sweep_src=src)
+        with torch.cuda.device(ing.table.device):
+            ing.table.copy_(self._table_staging, non_blocking=True)
+            self._table_copied.record()
+        self.last_h2d_bytes = self.pending_h2d_bytes + ing.table.numel()
+        self.pending_h2d_bytes = 0
+
+    def _graph_entry(self):
+        graphs = self.pipe._graphs
+        entry = graphs.get(self.key)
+        if entry is not None and entry.stream is self:
+            graphs.move_to_end(self.key)
+            return entry
+        graphs.pop(self.key, None)
+        while len(graphs) >= self.pipe.max_graphs:
+            graphs.popitem(last=False)
+        entry = graphs[self.key] = _StreamGraphEntry(self)
+        return entry
+
+    @torch.no_grad()
+    def infer(self, pinned_out=None, graphed=False):
+        """Detections of the current frame, host [B, D, nd+3] as infer_sweeps returns them, and bit-identical to
+        infer_sweeps(samples()).  The only H2D is the sweep table (the sweeps went with push).  graphed=True replays the
+        stream's CUDA graph.  On an f16-range overflow the model switches to tf32x3 and the same frame is re-run, as in
+        infer_sweeps; the history is not touched.  ValueError when a stream holds no sweep."""
+        self._stage_table()
+        pipe, ing = self.pipe, self._ingest
+        step = lambda: pipe.pack(pipe.forward_device(*ing.launch()))      # noqa: E731
+        for _attempt in range(2):
+            if graphed:         # (a re-run after an overflow captures a new graph: check_overflow dropped them all)
+                packed = pipe._run_graph(self._graph_entry(), step)
+            else:
+                packed = step()
+            pinned_out, rerun = pipe._fetch(packed, pinned_out)
+            if not rerun:
+                break
+        return pinned_out

@@ -16,6 +16,10 @@
 // the chunk prefix of the sweeps into shared memory (load_table); device tables are clamped there, the same way in every
 // CTA, before any point index is formed.  Chunks never straddle a sweep, so a CTA stages its sweep's transform once, and
 // one scan over the whole batch gives both the output rows and the per-sample cloud offsets.
+//
+// d3b_ingest_sweeps_gather adds one device array, sweep_src: the raw row where each sweep starts, so sweeps can be read
+// from wherever they sit (a ring of history slots) while sweep_offsets stays the logical prefix that drives the chunks,
+// the scan and the cloud offsets.  Without it the start of sweep s is its offset, which is the other two entry points.
 #include <climits>
 
 #include "common.cuh"
@@ -42,6 +46,7 @@ struct IngestParams {
   // device table (d3b_ingest_sweeps_dev), else nullptr
   const int* off_dev;
   const int* sample_dev;
+  const int* src_dev;                           // d3b_ingest_sweeps_gather only: raw row where each sweep starts
   const double* m_dev;                          // [n_sweeps][16]
   const float* lag_dev;
   const unsigned char* flags_dev;
@@ -49,7 +54,8 @@ struct IngestParams {
 
 // Per-CTA copy of the clamped table.
 struct IngestTable {
-  int off[kIngestMaxTable + 1];                 // raw rows of the sweeps
+  int off[kIngestMaxTable + 1];                 // logical prefix of the sweeps' lengths
+  int src[kIngestMaxTable];                     // raw row where each sweep starts (off[s] unless gathered)
   int chunk_off[kIngestMaxTable + 1];           // prefix of the sweeps' chunk counts
   int sample[kIngestMaxBatch + 1];              // sample b owns sweeps [sample[b], sample[b + 1])
   int buf[32];                                  // block-scan scratch
@@ -110,14 +116,30 @@ __device__ __forceinline__ bool clamp_table(Raw raw, int n, int cap, int* dst, i
   return bad;
 }
 
+constexpr int kClampedTable = 1, kClampedSrc = 2;   // status bits
+
 // Fills `t` from the params (host table) or from device memory (device table, clamped).  Returns, to every thread after
-// the barrier, whether the clamp changed anything.
-__device__ __forceinline__ bool load_table(const IngestParams& p, IngestTable& t) {
+// the barrier, which clamps changed anything (kClampedTable | kClampedSrc).
+__device__ __forceinline__ int load_table(const IngestParams& p, IngestTable& t) {
   bool bad = clamp_table([&](int i) { return p.off_dev != nullptr ? __ldg(p.off_dev + i) : p.off[i]; },
                          p.n_sweeps, p.raw_cap, t.off, t.chunk_off, t.buf);
   bad |= clamp_table([&](int b) { return p.sample_dev != nullptr ? __ldg(p.sample_dev + b) : (b == 0 ? 0 : p.n_sweeps); },
                      p.batch, p.n_sweeps, t.sample, nullptr, t.buf);
-  return __syncthreads_or(bad) != 0;
+  // t.off is complete here (the scans above passed barriers after writing it).  A gathered start is clamped into
+  // [0, raw_cap - len]; without sweep_src the start is the offset itself, which is always inside.
+  bool bad_src = false;
+  for (int s = threadIdx.x; s < p.n_sweeps; s += blockDim.x) {
+    const int off = t.off[s];
+    if (p.src_dev != nullptr) {
+      const int r = __ldg(p.src_dev + s), c = min(max(r, 0), p.raw_cap - (t.off[s + 1] - off));
+      bad_src |= c != r;
+      t.src[s] = c;
+    } else {
+      t.src[s] = off;
+    }
+  }
+  const int clamped = __syncthreads_or(bad) != 0 ? kClampedTable : 0;
+  return clamped | (__syncthreads_or(bad_src) != 0 ? kClampedSrc : 0);
 }
 
 // Chunks of the live sweeps (those of samples 0..batch-1); the rest of a capacity-sized grid returns.
@@ -169,7 +191,7 @@ ingest_count(const IngestParams p, const float* __restrict__ raw, int* __restric
   if (g >= live_chunks(p, t)) return;           // d3b_ingest_sweeps_dev: grid sized for the capacity
   const int s = sweep_of_chunk(p, t, g);
   const bool filter = (sweep_flags(p, s) & kFilterClose) != 0;
-  const int i0 = t.off[s] + (g - t.chunk_off[s]) * kIngestChunk + threadIdx.x * 4, end = t.off[s + 1];
+  const int i0 = t.src[s] + (g - t.chunk_off[s]) * kIngestChunk + threadIdx.x * 4, end = t.src[s] + t.off[s + 1] - t.off[s];
   int local = 0;
 #pragma unroll
   for (int j = 0; j < 4; ++j)
@@ -192,7 +214,7 @@ ingest_scan(const IngestParams p, const int* __restrict__ chunk_cnt, int* chunk_
             int out_cap, int* __restrict__ cloud_offsets, int* __restrict__ status) {
   __shared__ IngestTable t;
   __shared__ int running;
-  const bool clamped = load_table(p, t);
+  const int clamped = load_table(p, t);
   const int n_chunks = live_chunks(p, t);
   int* warp_sums = t.buf;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -227,7 +249,7 @@ ingest_scan(const IngestParams p, const int* __restrict__ chunk_cnt, int* chunk_
   }
   if (threadIdx.x == 0) {
     if (n_out != nullptr) *n_out = running < out_cap ? running : out_cap;
-    if (status != nullptr) *status = clamped ? 1 : 0;
+    if (status != nullptr) *status = clamped;
   }
   if (cloud_offsets != nullptr)
     for (int b = threadIdx.x; b <= p.batch; b += blockDim.x) {
@@ -250,7 +272,7 @@ ingest_emit(const IngestParams p, const float* __restrict__ raw, const int* __re
   const unsigned flags = sweep_flags(p, s);
   const float lag = p.lag_dev != nullptr ? __ldg(p.lag_dev + s) : p.time_lag[s];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int i0 = t.off[s] + (g - t.chunk_off[s]) * kIngestChunk + threadIdx.x * 4, end = t.off[s + 1];
+  const int i0 = t.src[s] + (g - t.chunk_off[s]) * kIngestChunk + threadIdx.x * 4, end = t.src[s] + t.off[s + 1] - t.off[s];
   unsigned int kept = 0u;
 #pragma unroll
   for (int j = 0; j < 4; ++j)
@@ -353,32 +375,60 @@ extern "C" int d3b_ingest_sweeps(const float* raw, const int32_t* sweep_offsets,
                        (int*)((char*)workspace + need / 2), stream);
 }
 
+namespace {
+
+// d3b_ingest_sweeps_dev and d3b_ingest_sweeps_gather: the same checks and launches, sweep_src = nullptr for the former.
+int ingest_dev(const char* name, const float* raw, int32_t raw_capacity, int32_t raw_stride, int32_t n_feat,
+               const int32_t* sweep_offsets, const int32_t* sweep_src, const int32_t* sample_sweeps,
+               const double* transforms, const float* time_lag, const uint8_t* flags, int32_t sweep_capacity,
+               int32_t batch, float radius, float* out, int32_t* cloud_offsets, int32_t* status, void* workspace,
+               size_t workspace_bytes, cudaStream_t stream) {
+  D3B_REQUIRE(sweep_offsets && sample_sweeps && transforms && time_lag && flags && cloud_offsets && workspace,
+              "%s: null argument", name);
+  D3B_REQUIRE(batch >= 1 && batch <= kIngestMaxBatch, "%s: batch %d outside [1, %d]", name, batch, kIngestMaxBatch);
+  D3B_REQUIRE(sweep_capacity >= 1 && sweep_capacity <= D3B_INGEST_MAX_SWEEPS * batch,
+              "%s: sweep_capacity %d outside [1, %d * batch]", name, sweep_capacity, D3B_INGEST_MAX_SWEEPS);
+  D3B_REQUIRE(raw_capacity >= 0 && raw_capacity <= (1 << 30), "%s: raw_capacity %d outside [0, 2^30]", name,
+              raw_capacity);
+  D3B_REQUIRE(n_feat >= 3 && raw_stride >= n_feat, "%s: bad layout (n_feat %d, stride %d)", name, n_feat, raw_stride);
+  D3B_REQUIRE(raw_capacity == 0 || (raw && out), "%s: null buffer", name);
+  const size_t need = d3b_ingest_dev_workspace_bytes(raw_capacity, sweep_capacity);
+  if (need > workspace_bytes) {
+    set_error("%s: workspace %zu < %zu", name, workspace_bytes, need);
+    return D3B_ERR_WORKSPACE;
+  }
+  IngestParams p = params_of(sweep_capacity, batch, raw_stride, n_feat, radius);
+  p.raw_cap = raw_capacity;
+  p.off_dev = sweep_offsets; p.src_dev = sweep_src; p.sample_dev = sample_sweeps; p.m_dev = transforms;
+  p.lag_dev = time_lag; p.flags_dev = flags;
+  return launch_ingest(p, raw, div_up(raw_capacity, kIngestChunk) + sweep_capacity, out, raw_capacity, nullptr,
+                       cloud_offsets, status, (int*)workspace, (int*)((char*)workspace + need / 2), stream);
+}
+
+}  // namespace
+
 extern "C" int d3b_ingest_sweeps_dev(const float* raw, int32_t raw_capacity, int32_t raw_stride, int32_t n_feat,
                                      const int32_t* sweep_offsets, const int32_t* sample_sweeps, const double* transforms,
                                      const float* time_lag, const uint8_t* flags, int32_t sweep_capacity, int32_t batch,
                                      float radius, float* out, int32_t* cloud_offsets, int32_t* status, void* workspace,
                                      size_t workspace_bytes, void* stream_) {
-  D3B_REQUIRE(sweep_offsets && sample_sweeps && transforms && time_lag && flags && cloud_offsets && workspace,
-              "d3b_ingest_sweeps_dev: null argument");
-  D3B_REQUIRE(batch >= 1 && batch <= kIngestMaxBatch, "d3b_ingest_sweeps_dev: batch %d outside [1, %d]", batch,
-              kIngestMaxBatch);
-  D3B_REQUIRE(sweep_capacity >= 1 && sweep_capacity <= D3B_INGEST_MAX_SWEEPS * batch,
-              "d3b_ingest_sweeps_dev: sweep_capacity %d outside [1, %d * batch]", sweep_capacity, D3B_INGEST_MAX_SWEEPS);
-  D3B_REQUIRE(raw_capacity >= 0 && raw_capacity <= (1 << 30), "d3b_ingest_sweeps_dev: raw_capacity %d outside [0, 2^30]",
-              raw_capacity);
-  D3B_REQUIRE(n_feat >= 3 && raw_stride >= n_feat, "d3b_ingest_sweeps_dev: bad layout (n_feat %d, stride %d)", n_feat,
-              raw_stride);
-  D3B_REQUIRE(raw_capacity == 0 || (raw && out), "d3b_ingest_sweeps_dev: null buffer");
-  const size_t need = d3b_ingest_dev_workspace_bytes(raw_capacity, sweep_capacity);
-  if (need > workspace_bytes) {
-    set_error("d3b_ingest_sweeps_dev: workspace %zu < %zu", workspace_bytes, need);
-    return D3B_ERR_WORKSPACE;
-  }
-  IngestParams p = params_of(sweep_capacity, batch, raw_stride, n_feat, radius);
-  p.raw_cap = raw_capacity;
-  p.off_dev = sweep_offsets; p.sample_dev = sample_sweeps; p.m_dev = transforms; p.lag_dev = time_lag;
-  p.flags_dev = flags;
-  return launch_ingest(p, raw, div_up(raw_capacity, kIngestChunk) + sweep_capacity, out, raw_capacity, nullptr,
-                       cloud_offsets, status, (int*)workspace, (int*)((char*)workspace + need / 2),
-                       (cudaStream_t)stream_);
+  return ingest_dev("d3b_ingest_sweeps_dev", raw, raw_capacity, raw_stride, n_feat, sweep_offsets, nullptr,
+                    sample_sweeps, transforms, time_lag, flags, sweep_capacity, batch, radius, out, cloud_offsets, status,
+                    workspace, workspace_bytes, (cudaStream_t)stream_);
+}
+
+extern "C" size_t d3b_ingest_gather_workspace_bytes(int32_t raw_capacity, int32_t sweep_capacity) {
+  return d3b_ingest_dev_workspace_bytes(raw_capacity, sweep_capacity);
+}
+
+extern "C" int d3b_ingest_sweeps_gather(const float* raw, int32_t raw_capacity, int32_t raw_stride, int32_t n_feat,
+                                        const int32_t* sweep_offsets, const int32_t* sweep_src,
+                                        const int32_t* sample_sweeps, const double* transforms, const float* time_lag,
+                                        const uint8_t* flags, int32_t sweep_capacity, int32_t batch, float radius,
+                                        float* out, int32_t* cloud_offsets, int32_t* status, void* workspace,
+                                        size_t workspace_bytes, void* stream_) {
+  D3B_REQUIRE(sweep_src, "d3b_ingest_sweeps_gather: null argument (sweep_src)");
+  return ingest_dev("d3b_ingest_sweeps_gather", raw, raw_capacity, raw_stride, n_feat, sweep_offsets, sweep_src,
+                    sample_sweeps, transforms, time_lag, flags, sweep_capacity, batch, radius, out, cloud_offsets, status,
+                    workspace, workspace_bytes, (cudaStream_t)stream_);
 }

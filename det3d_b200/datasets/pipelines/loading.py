@@ -12,8 +12,14 @@ voxelizer consumes directly (no second H2D copy).
 `ingest_sweeps_batched` does the same for a batch of samples in one d3b_ingest_sweeps_dev call: the sweep table lives
 in device memory and the per-sample cloud offsets stay there, in the form the voxelizer's device-offset path takes, so
 nothing between the raw sweeps and the detections waits on the host (InferencePipeline.infer_sweeps).
+
+`BatchedIngest(gather=True)` runs d3b_ingest_sweeps_gather instead: the table also says at which raw row each sweep
+starts, so sweeps are read where they already lie in device memory (the history slots of apis.SweepStream), and
+`stream_transforms` gives the float64 key-frame transforms and lags of such a history.
 """
+import collections
 import ctypes as C
+import numbers
 from pathlib import Path
 
 import numpy as np
@@ -129,12 +135,14 @@ def sweep_table_capacity(n_sweeps, batch):
     return min(1 << (max(int(n_sweeps), 1) - 1).bit_length(), MAX_SWEEPS * batch)
 
 
-def sweep_table_views(buf, sweep_capacity, batch):
+def sweep_table_views(buf, sweep_capacity, batch, gather=False):
     """Typed views over one byte buffer (numpy or torch) holding a device sweep table, laid out as
-    transforms f64 [S, 16] | sweep_offsets i32 [S + 1] | sample_sweeps i32 [B + 1] | time_lag f32 [S] | flags u8 [S]."""
+    transforms f64 [S, 16] | sweep_offsets i32 [S + 1] | sample_sweeps i32 [B + 1] | time_lag f32 [S] | flags u8 [S],
+    with sweep_src i32 [S] after sample_sweeps when `gather`."""
     S, B = sweep_capacity, batch
-    parts, views, at = (("transforms", 8, S * 16), ("sweep_offsets", 4, S + 1), ("sample_sweeps", 4, B + 1),
-                        ("time_lag", 4, S), ("flags", 1, S)), {}, 0
+    parts = (("transforms", 8, S * 16), ("sweep_offsets", 4, S + 1), ("sample_sweeps", 4, B + 1)) \
+        + ((("sweep_src", 4, S),) if gather else ()) + (("time_lag", 4, S), ("flags", 1, S))
+    views, at = {}, 0
     is_np = isinstance(buf, np.ndarray)
     for name, size, count in parts:
         raw = buf[at:at + size * count]
@@ -147,8 +155,8 @@ def sweep_table_views(buf, sweep_capacity, batch):
 _TORCH_DTYPE = {np.float64: torch.float64, np.float32: torch.float32, np.int32: torch.int32, np.uint8: torch.uint8}
 
 
-def sweep_table_bytes(sweep_capacity, batch):
-    return sweep_capacity * (16 * 8 + 4 + 4 + 1) + 4 * (batch + 2)
+def sweep_table_bytes(sweep_capacity, batch, gather=False):
+    return sweep_capacity * (16 * 8 + 4 + 4 + 1 + (4 if gather else 0)) + 4 * (batch + 2)
 
 
 def fill_sweep_table(views, samples, sizes):
@@ -174,6 +182,60 @@ def fill_sweep_table(views, samples, sizes):
     views["sweep_offsets"][s + 1:] = rows         # unused table rows: empty sweeps past the last sample
 
 
+def stream_transforms(poses, timestamps):
+    """Key-frame transforms and time lags of one sweep history, newest (the key frame) first: poses are sensor-to-world
+    4x4 float64 matrices, timestamps in seconds.  Sweep s > 0 gets inv(P_key) @ P_s in float64 (its points to the key
+    frame's sensor frame), the key frame None; lags are t_key - t_s (the table rounds them to float32 once).  Returns
+    (transforms, time_lags) in ingest_sweeps' form."""
+    key_inv = np.linalg.inv(np.asarray(poses[0], np.float64))
+    tms = [None] + [key_inv @ np.asarray(p, np.float64) for p in poses[1:]]
+    t_key = float(timestamps[0])
+    return tms, [t_key - float(t) for t in timestamps]
+
+
+class SweepHistory:
+    """Host bookkeeping of B sweep histories of K slots each (apis.SweepStream keeps the sweeps themselves on the
+    device).  A push goes to slot (pushes since the last reset) mod K of its stream, so the slot it overwrites is the
+    stream's oldest once K sweeps are held; reset(b) forgets stream b's sweeps."""
+
+    def __init__(self, batch, history):
+        self.batch, self.history = batch, history
+        self.count = [0] * batch                  # pushes since the last reset
+        # per stream, oldest first: (slot, rows, pose f64 [4, 4], timestamp) of the sweeps still held
+        self.held = [collections.deque(maxlen=history) for _ in range(batch)]
+
+    def check_stream(self, b):
+        if not isinstance(b, numbers.Integral) or not 0 <= b < self.batch:
+            raise ValueError("stream index %r outside [0, %d)" % (b, self.batch))
+
+    def next_slot(self, b):
+        return self.count[b] % self.history
+
+    def record(self, b, rows, pose, timestamp):
+        """Books stream b's new sweep into next_slot(b), which it returns."""
+        slot = self.next_slot(b)
+        self.held[b].append((slot, int(rows), np.array(pose, dtype=np.float64), float(timestamp)))
+        self.count[b] += 1
+        return slot
+
+    def reset(self, b):
+        self.check_stream(b)
+        self.count[b] = 0
+        self.held[b].clear()
+
+    def frame(self):
+        """The current frame: per stream (slots, rows, transforms, time_lags), newest sweep (the key frame) first, with
+        stream_transforms' transforms and lags.  ValueError when a stream holds no sweep."""
+        out = []
+        for b, held in enumerate(self.held):
+            if not held:
+                raise ValueError("stream %d has no sweep: push one before inferring" % b)
+            newest = list(reversed(held))
+            tms, lags = stream_transforms([h[2] for h in newest], [h[3] for h in newest])
+            out.append(([h[0] for h in newest], [h[1] for h in newest], tms, lags))
+        return out
+
+
 def stage_raw_sweeps(samples, sizes, raw_dev, staging=None):
     """Enqueues the H2D copies of every raw sweep into raw_dev, back to back in sample order.  Pinned tensors are copied
     directly; anything else goes through the pinned `staging` buffer ([>= total, raw_stride], allocated when None)."""
@@ -195,38 +257,50 @@ def stage_raw_sweeps(samples, sizes, raw_dev, staging=None):
 class BatchedIngest:
     """Device buffers of one batched-ingest shape -- raw [raw_capacity, raw_stride], the sweep table, the ingested
     clouds [raw_capacity, n_feat + 1], cloud_offsets [B + 1], status, workspace -- and the d3b_ingest_sweeps_dev call
-    over them.  The addresses never change, so a captured CUDA graph can hold them."""
+    over them.  The addresses never change, so a captured CUDA graph can hold them.  With `gather` the table also holds
+    sweep_src (the raw row where each sweep starts) and launch() runs d3b_ingest_sweeps_gather."""
 
-    def __init__(self, batch, raw_capacity, sweep_capacity, raw_stride, n_feat=4, radius=1.0, device="cuda"):
+    def __init__(self, batch, raw_capacity, sweep_capacity, raw_stride, n_feat=4, radius=1.0, device="cuda",
+                 gather=False):
         dev = torch.device(device)
         self.batch, self.raw_capacity, self.sweep_capacity = batch, raw_capacity, sweep_capacity
-        self.raw_stride, self.n_feat, self.radius = raw_stride, n_feat, radius
-        self.raw = torch.empty((raw_capacity, raw_stride), dtype=torch.float32, device=dev)   # rows past the live total are never read
-        self.table = torch.zeros(sweep_table_bytes(sweep_capacity, batch), dtype=torch.uint8, device=dev)
-        self.tables = sweep_table_views(self.table, sweep_capacity, batch)
+        self.raw_stride, self.n_feat, self.radius, self.gather = raw_stride, n_feat, radius, gather
+        self.raw = torch.empty((raw_capacity, raw_stride), dtype=torch.float32, device=dev)   # rows no sweep covers are never read
+        self.table = torch.zeros(sweep_table_bytes(sweep_capacity, batch, gather), dtype=torch.uint8, device=dev)
+        self.tables = sweep_table_views(self.table, sweep_capacity, batch, gather)
         self.out = torch.empty((raw_capacity, n_feat + 1), dtype=torch.float32, device=dev)
         self.cloud_offsets = torch.zeros(batch + 1, dtype=torch.int32, device=dev)
         self.status = torch.zeros(1, dtype=torch.int32, device=dev)
         self.ws = torch.empty(_lib.lib().d3b_ingest_dev_workspace_bytes(raw_capacity, sweep_capacity), dtype=torch.uint8,
                               device=dev)
 
-    def host_table(self, samples, sizes, out=None):
-        """The table image of `samples` as uint8 host bytes (into `out`, e.g. a pinned buffer, when given)."""
+    def host_table(self, samples, sizes, out=None, sweep_src=None):
+        """The table image of `samples` as uint8 host bytes (into `out`, e.g. a pinned buffer, when given).  A gather
+        table takes sweep_src, the raw start row of every sweep in sample order (unused rows stay 0)."""
         buf = np.zeros(self.table.numel(), np.uint8) if out is None else out
-        fill_sweep_table(sweep_table_views(buf, self.sweep_capacity, self.batch), samples, sizes)
+        views = sweep_table_views(buf, self.sweep_capacity, self.batch, self.gather)
+        fill_sweep_table(views, samples, sizes)
+        if self.gather:
+            src = np.asarray([] if sweep_src is None else sweep_src, np.int64)
+            if src.shape != (sum(map(len, sizes)),):
+                raise ValueError("a gather table needs one sweep_src per sweep (%d), got %s"
+                                 % (sum(map(len, sizes)), src.shape))
+            views["sweep_src"][:src.shape[0]] = src
         return buf
 
     def launch(self):
         """Ingests the raw sweeps under the device table into out / cloud_offsets (three kernels, no host sync)."""
         t = self.tables
+        L, name = _lib.lib(), "d3b_ingest_sweeps_gather" if self.gather else "d3b_ingest_sweeps_dev"
+        head = (self.raw.data_ptr(), self.raw_capacity, self.raw_stride, self.n_feat, t["sweep_offsets"].data_ptr())
+        head += (t["sweep_src"].data_ptr(),) if self.gather else ()
         with _lib.on_device_of(self.raw), _lib.timed("ingest_sweeps", batch=self.batch, capacity=self.raw_capacity):
-            st = _lib.lib().d3b_ingest_sweeps_dev(
-                self.raw.data_ptr(), self.raw_capacity, self.raw_stride, self.n_feat, t["sweep_offsets"].data_ptr(),
-                t["sample_sweeps"].data_ptr(), t["transforms"].data_ptr(), t["time_lag"].data_ptr(),
+            st = getattr(L, name)(
+                *head, t["sample_sweeps"].data_ptr(), t["transforms"].data_ptr(), t["time_lag"].data_ptr(),
                 t["flags"].data_ptr(), self.sweep_capacity, self.batch, C.c_float(self.radius), self.out.data_ptr(),
                 self.cloud_offsets.data_ptr(), self.status.data_ptr(), self.ws.data_ptr(), self.ws.numel(),
                 _lib.current_stream())
-        _lib.check(st, "d3b_ingest_sweeps_dev")
+        _lib.check(st, name)
         return self.out, self.cloud_offsets
 
 

@@ -133,6 +133,23 @@ int d3b_ingest_sweeps_dev(const float* raw, int32_t raw_capacity, int32_t raw_st
                           float radius, float* out, int32_t* cloud_offsets, int32_t* status, void* workspace,
                           size_t workspace_bytes, void* stream);
 
+/* d3b_ingest_sweeps_dev with each sweep read from wherever it lies in `raw` (e.g. a ring of per-stream history slots that
+ * stay on the device from one frame to the next).  Same arguments, plus
+ * sweep_src      [S] i32 DEVICE: sweep s is rows [sweep_src[s], sweep_src[s] + len_s) of raw, len_s = sweep_offsets[s + 1] -
+ *                sweep_offsets[s]; rows no sweep covers are never read
+ * sweep_offsets keeps its role as the logical prefix of the sweeps' lengths: it drives the chunking, the scan and
+ * cloud_offsets, so `out` / cloud_offsets are laid out exactly as d3b_ingest_sweeps_dev's, and its bound is still
+ * sweep_offsets[S] <= raw_capacity.  After the offsets are clamped, each sweep_src[s] is clamped into
+ * [0, raw_capacity - len_s], identically in every CTA, before any point index is formed; status bit 1 (value 2) is set
+ * when that changed anything, bit 0 (value 1) keeps its meaning.  With sweep_src[s] = sweep_offsets[s] the results are
+ * d3b_ingest_sweeps_dev's, bit for bit.  workspace: d3b_ingest_gather_workspace_bytes(raw_capacity, S). */
+size_t d3b_ingest_gather_workspace_bytes(int32_t raw_capacity, int32_t sweep_capacity);
+int d3b_ingest_sweeps_gather(const float* raw, int32_t raw_capacity, int32_t raw_stride, int32_t n_feat,
+                             const int32_t* sweep_offsets, const int32_t* sweep_src, const int32_t* sample_sweeps,
+                             const double* transforms, const float* time_lag, const uint8_t* flags,
+                             int32_t sweep_capacity, int32_t batch, float radius, float* out, int32_t* cloud_offsets,
+                             int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ========================================================================= *
  * 2. Rulebook (sparse-convolution index maps)
  *    replaces spconv v1.x `get_indice_pairs` as called by SubMConv3d /
