@@ -6,16 +6,20 @@
 //   (det3d/core/bbox/box_torch_ops.py:80-148) -> rotated NMS (-> csrc/nms.cu) ->
 //   direction fix -> post_center_limit_range mask,
 // as six launches over fixed-size buffers:
-//   P1 head_scores     best logit / label per anchor straight from the (possibly strided) head rows
+//   P1 head_scores     label (first class with the maximal fp32 score) and its logit per anchor, straight from the
+//                      (possibly strided) head rows
 //   P2 topk            histogram of the leading key bits (built inside P1) -> partition kernel appends the pivot
 //                      bin and everything above it to a candidate list -> one CTA per sample sorts the list
 //                      (value desc, index asc) in shared memory and emits the first k
-//   P3 decode_selected decode ONLY the k selected anchors (the reference decodes all 70,400),
-//                      sigmoid, direction label, count of scores >= threshold (a prefix, scores are sorted)
-//   -- d3b_rotate_nms / d3b_normal_nms on the k candidates (n_valid read on the device) --
+//   P3 decode_selected sigmoid of the k selected anchors, compaction of those with score >= threshold (n_valid),
+//                      decode of those only (the reference decodes all 70,400), direction label
+//   -- d3b_rotate_nms / d3b_normal_nms on the n_valid candidates (n_valid read on the device) --
 //   P4 finalize        gather the kept boxes, direction flip, range mask -> packed [B, post, nd+3] rows
-// Selection is identical to the reference's "filter, then top-k": sigmoid is monotonic, so the
-// passing set is a prefix of the top-k by logit.
+// Selection matches the reference's "filter, then top-k" because sigmoid is nondecreasing: the passing anchors are the
+// ones with the highest logits.  P3 still tests every selected candidate against the threshold instead of assuming a
+// prefix, so the set entering NMS is exactly {score >= threshold} even where the rounding of expf is not monotonic.
+// Ties in the logit go to the lower anchor index; -0 counts as +0; an anchor with a NaN logit in any class ranks
+// below all others and never passes a positive threshold.
 #include <algorithm>
 
 #include "common.cuh"
@@ -37,6 +41,13 @@ __device__ __forceinline__ unsigned int float_to_ordered(float f) {
 constexpr int kTopkBinBits = 11;
 constexpr int kTopkBins = 1 << kTopkBinBits;
 
+// torch.sigmoid in fp32: the same expression wherever a score is compared or stored
+__device__ __forceinline__ float sigmoid_rn(float x) { return __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-x))); }
+
+// The key of an anchor whose logits hold a NaN: a negative NaN whose ordered key is 0, below every other value
+// (-inf included), so it is selected only when fewer than k other anchors exist and never passes a threshold.
+constexpr unsigned int kNanKeyBits = 0xffffffffu;
+
 __global__ void __launch_bounds__(256)
 head_scores_kernel(const float* __restrict__ cls, int row_stride, int col0, int hw, int na, int n_cls,
                    float* __restrict__ best_logit, unsigned char* __restrict__ best_label,
@@ -48,12 +59,23 @@ head_scores_kernel(const float* __restrict__ cls, int row_stride, int col0, int 
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < A; i += gridDim.x * blockDim.x) {
     const int cell = i / na, a = i - cell * na;
     const float* p = cls + ((size_t)b * hw + cell) * row_stride + col0 + a * n_cls;
+    // mg_head.py:993: torch.max over the fp32 sigmoid SCORES, first maximum wins.  Distinct logits can share a score
+    // (both 1.0f once saturated), so the label is chosen on the scores; the key is the chosen class's logit, whose
+    // score is the top score.  A NaN anywhere makes torch.max return NaN, which never passes `>= threshold`.
     float best = p[0];
+    bool nan = isnan(best);
     int lab = 0;
-    for (int c = 1; c < n_cls; ++c) {
-      const float v = p[c];
-      if (v > best) { best = v; lab = c; }    // first maximum wins, like torch.max
+    if (n_cls > 1) {
+      float best_s = sigmoid_rn(best);
+      for (int c = 1; c < n_cls; ++c) {
+        const float v = p[c];
+        nan |= isnan(v);
+        const float s = sigmoid_rn(v);
+        if (s > best_s) { best_s = s; best = v; lab = c; }
+      }
     }
+    // -0 and +0 are one logit: without this every +0 would outrank every -0 in the ordered key, whatever the index
+    best = nan ? __uint_as_float(kNanKeyBits) : __fadd_rn(best, 0.0f);
     best_logit[(size_t)b * A + i] = best;
     best_label[(size_t)b * A + i] = (unsigned char)lab;
     atomicAdd(&s_hist[float_to_ordered(best) >> (32 - kTopkBinBits)], 1u);
@@ -267,15 +289,45 @@ struct PredictDev {
   int has_range, label_offset;
 };
 
-__global__ void __launch_bounds__(256)
+// grid = (chunks of kDecodeThreads candidates, batch).  The candidates arrive in selection order; those whose score
+// passes the threshold are compacted, in that order, to the front of the sample's slots (n_valid of them), and only
+// they are decoded.  The passing set is exactly {score >= threshold} even where fp32 sigmoid is not monotonic in the
+// logit, so it need not be a prefix of the selection.  A CTA finds its chunk's first slot by testing the chunks before
+// it (one sigmoid per candidate, <= 7 rounds at k = 2048), so the decode stays spread over the SMs at batch 1.
+constexpr int kDecodeThreads = 256;
+
+__device__ __forceinline__ bool candidate_passes(const PredictDev& p, const float* sel_logit, int b, int j, float* sc) {
+  const float s = sigmoid_rn(sel_logit[(size_t)b * p.k + j]);
+  if (sc) *sc = s;
+  return !(p.score_thr > 0.0f) || s >= p.score_thr;
+}
+
+__global__ void __launch_bounds__(kDecodeThreads)
 decode_selected_kernel(PredictDev p, const float* __restrict__ sel_logit, const int* __restrict__ sel_idx,
                        float* __restrict__ cand, float* __restrict__ nms_boxes, float* __restrict__ scores,
                        int* __restrict__ labels, int* __restrict__ dir_labels, int* __restrict__ n_valid) {
+  __shared__ int s_warp[kDecodeThreads / 32];
   const int A = p.hw * p.na;
-  const int total = p.batch * p.k;
-  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < total; e += gridDim.x * blockDim.x) {
-    const int b = e / p.k;
-    const int i = sel_idx[e];
+  const int b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  int base = 0;
+  for (int r = 0; r < (int)blockIdx.x; ++r)                     // every candidate of these chunks exists (j < k)
+    base += __syncthreads_count(candidate_passes(p, sel_logit, b, r * kDecodeThreads + tid, nullptr));
+  const int j = blockIdx.x * kDecodeThreads + tid;
+  float sc = 0.0f;
+  const bool pass = j < p.k && candidate_passes(p, sel_logit, b, j, &sc);
+  const unsigned int bal = __ballot_sync(0xffffffffu, pass);
+  if (lane == 0) s_warp[warp] = __popc(bal);
+  __syncthreads();
+  int before = 0, total = 0;
+  for (int w = 0; w < kDecodeThreads / 32; ++w) {               // broadcast reads
+    const int c = s_warp[w];
+    before += w < warp ? c : 0;
+    total += c;
+  }
+  if (tid == 0 && blockIdx.x == gridDim.x - 1) n_valid[b] = base + total;
+  if (pass) {
+    const int e = b * p.k + base + before + __popc(bal & ((1u << lane) - 1u));
+    const int i = sel_idx[(size_t)b * p.k + j];
     const int cell = i / p.na, a = i - cell * p.na;
     const float* t = p.box + ((size_t)b * p.hw + cell) * p.box_stride + p.box_col0 + a * p.code;
     const float* an = p.anchors + (size_t)i * p.nd;
@@ -320,14 +372,12 @@ decode_selected_kernel(PredictDev p, const float* __restrict__ sel_logit, const 
       }
       nb[0] = mnx; nb[1] = mny; nb[2] = mxx; nb[3] = mxy; nb[4] = 0.0f;
     }
-    const float sc = __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-sel_logit[e])));   // torch.sigmoid in fp32
     scores[e] = sc;
     labels[e] = (int)p.best_label[(size_t)b * A + i] + p.label_offset;
     if (p.dir != nullptr) {
       const float* d = p.dir + ((size_t)b * p.hw + cell) * p.dir_stride + p.dir_col0 + a * 2;
       dir_labels[e] = d[1] > d[0] ? 1 : 0;                            // torch.max: first maximum wins
     }
-    if (!(p.score_thr > 0.0f) || sc >= p.score_thr) atomicAdd(&n_valid[b], 1);
   }
 }
 
@@ -352,7 +402,8 @@ finalize_kernel(PredictDev p, const float* __restrict__ cand, const float* __res
     for (int c = 0; c < p.nd; ++c) o[c] = bx[c];
     if (p.dir != nullptr) {
       const bool opp = ((bx[p.nd - 1] - p.direction_offset) > 0.0f) != (dir_labels[src] != 0);   // mg_head.py:1044-1051
-      if (opp) o[p.nd - 1] = __fadd_rn(bx[p.nd - 1], 3.14159265358979323846f);
+      // the reference adds torch.where(opp, pi, 0) to every angle: an angle of -0 comes out +0 when not flipped
+      o[p.nd - 1] = __fadd_rn(bx[p.nd - 1], opp ? 3.14159265358979323846f : 0.0f);
     }
     bool ok = true;
     if (p.has_range) {
@@ -454,8 +505,7 @@ extern "C" int d3b_predict_task(const d3b_predict_params* q, float* packed, int3
   topk_finish_kernel<<<dim3(kTopkFinishCtas, q->batch), kTopkThreads, kTopkSortCap * 8, stream>>>(w.part, w.part_count, A, q->pre_max,
                                                                           w.sel_logit, w.sel_idx);
   D3B_LAUNCH_CHECK();
-  D3B_CUDA(cudaMemsetAsync(w.n_valid, 0, (size_t)q->batch * 4, stream));
-  decode_selected_kernel<<<grid_for((long long)q->batch * q->pre_max, 256), 256, 0, stream>>>(
+  decode_selected_kernel<<<dim3((unsigned)div_up(q->pre_max, kDecodeThreads), (unsigned)q->batch), kDecodeThreads, 0, stream>>>(
       p, w.sel_logit, w.sel_idx, w.cand, w.nms_boxes, w.scores, w.labels, w.dir_labels, w.n_valid);
   D3B_LAUNCH_CHECK();
   // one NMS per sample, all samples in the same two launches (mask, sweep)

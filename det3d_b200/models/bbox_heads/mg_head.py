@@ -150,7 +150,9 @@ class MultiGroupHead(nn.Module):
         if C == 1:
             top_logit, top_labels = logits.squeeze(-1), None
         else:
-            top_logit, top_labels = torch.max(logits, dim=-1)
+            # mg_head.py:993: the label is the first class with the maximal fp32 SCORE (distinct logits can share one)
+            top_labels = torch.max(torch.sigmoid(logits), dim=-1)[1]
+            top_logit = torch.gather(logits, -1, top_labels.unsqueeze(-1)).squeeze(-1)
         sel_logit, sel_idx = torch.topk(top_logit, k=pre, dim=1)                 # descending
         sel_scores = torch.sigmoid(sel_logit)
         if thr > 0.0:
