@@ -153,7 +153,7 @@ SIGNATURES = {
     "d3b_sparse_conv16": (C.c_int, [_vp, _vp, _vp, _i32, C.POINTER(Conv16Params), _vp]),
     "d3b_split16": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _vp]),
     "d3b_merge16": (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
-    "d3b_sparse_to_bev16": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _I3, _i32, _vp, _vp, _vp]),
+    "d3b_sparse_to_bev16": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _I3, _i32, _vp, _vp, _vp, _vp]),
     "d3b_bev_conv16": (C.c_int, [C.POINTER(Bev16Params), _vp]),
     "d3b_predict_workspace_bytes": (_sz, [C.POINTER(PredictParams)]),
     "d3b_predict_task": (C.c_int, [C.POINTER(PredictParams), _vp, _i32, _i32, _vp, _vp, _sz, _vp]),

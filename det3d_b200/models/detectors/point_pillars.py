@@ -33,7 +33,8 @@ class PointPillars(_FusedBevMixin, SingleStageDetector):
             kw = {} if data["n_dev"] is None else {"n_dev": data["n_dev"]}
             feats = self._read(data)
             ovf = self.overflow_flag(feats.device)
-            planes = self.backbone.forward_planes(feats, data["coors"], data["batch_size"], data["input_shape"], **kw)
+            planes = self.backbone.forward_planes(feats, data["coors"], data["batch_size"], data["input_shape"],
+                                                  overflow=ovf, **kw)
             preds = bev.run(planes, overflow=ovf)
         else:
             preds = self.bbox_head(self.extract_feat(data))

@@ -165,9 +165,10 @@ class PointPillarsScatter(nn.Module):
     def init_weights(self, pretrained=None):
         pass
 
-    def forward_planes(self, voxel_features, coords, batch_size, input_shape, n_dev=None):
+    def forward_planes(self, voxel_features, coords, batch_size, input_shape, n_dev=None, overflow=None):
         """[M, C] pillar features + coords -> NHWC split-f16 planes [B, ny, nx, C] (the FP16x3 dense path's input);
-        the canvas of pillar_encoder.py:175-211 in channels-last layout, split on the way."""
+        the canvas of pillar_encoder.py:175-211 in channels-last layout, split on the way.  A feature outside the f16
+        range ORs 1 into `overflow` (int32[1] device flag, or None)."""
         from det3d_b200.ops.spconv import conv16, core
         nx, ny = int(input_shape[0]), int(input_shape[1])
         feats = voxel_features.to(torch.float32).contiguous()
@@ -185,7 +186,7 @@ class PointPillarsScatter(nn.Module):
         out.zero_()
         if m > 0:
             level = core.SparseLevel(coords, n, m, (1, ny, nx), batch_size)
-            conv16.sparse_to_bev16(feats, level, out)
+            conv16.sparse_to_bev16(feats, level, out, overflow=overflow)
         return out
 
     def forward(self, voxel_features, coords, batch_size, input_shape, n_dev=None):

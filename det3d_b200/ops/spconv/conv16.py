@@ -150,8 +150,9 @@ def sparse_conv16(x, rb, cw, out, residual=None, out_f32=None, overflow=None, ta
     return out
 
 
-def sparse_to_bev16(x, level, out):
-    """Sparse rows (Planes [cap, C] or fp32 [cap, C]) -> zero-filled NHWC planes `out` [B, H, W, C*D], channel = c*D+z."""
+def sparse_to_bev16(x, level, out, overflow=None):
+    """Sparse rows (Planes [cap, C] or fp32 [cap, C]) -> zero-filled NHWC planes `out` [B, H, W, C*D], channel = c*D+z.
+    fp32 rows are split on the way: one outside the f16 range ORs 1 into `overflow` (int32[1] device flag, or None)."""
     c = x.shape[-1]
     hi = lo = f32 = None
     if isinstance(x, Planes):
@@ -162,7 +163,8 @@ def sparse_to_bev16(x, level, out):
     sp = (C.c_int32 * 3)(*[int(v) for v in level.spatial])
     with _lib.on_device_of(dev_t):
         st = _lib.lib().d3b_sparse_to_bev16(hi, lo, f32, level.coors.data_ptr(), level.n.data_ptr(), level.cap, c, sp,
-                                            level.batch, out.hi.data_ptr(), out.lo.data_ptr(), _lib.current_stream())
+                                            level.batch, out.hi.data_ptr(), out.lo.data_ptr(), _lib.ptr(overflow),
+                                            _lib.current_stream())
     _lib.check(st, "d3b_sparse_to_bev16")
     return out
 

@@ -353,12 +353,14 @@ int d3b_sparse_conv16(const int32_t* nbr, const uint32_t* tile_mask, const int32
                       const d3b_conv16_params* p, void* stream);
 
 /* fp32 <-> plane conversions (API boundaries) and the sparse -> dense NHWC scatter on planes
- * (channel = c*D + z, as d3b_sparse_to_bev_rows; rows given as planes OR as fp32). */
+ * (channel = c*D + z, as d3b_sparse_to_bev_rows; rows given as planes OR as fp32).  Every launch that splits fp32
+ * values into planes ORs 1 into `*overflow` (may be NULL) when one of them has |x| >= 65504 or is NaN: d3b_split16
+ * and d3b_sparse_to_bev16 with fp32 rows.  Plane rows are copied as they are (their writer checked them). */
 int d3b_split16(const float* x, int64_t n, void* hi, void* lo, int32_t* overflow, void* stream);
 int d3b_merge16(const void* hi, const void* lo, int64_t n, float* x, void* stream);
 int d3b_sparse_to_bev16(const void* in_hi, const void* in_lo, const float* in_f32, const int32_t* coors,
                         const int32_t* n_rows, int32_t row_cap, int32_t channels, const int32_t spatial[3],
-                        int32_t batch, void* out_hi, void* out_lo, void* stream);
+                        int32_t batch, void* out_hi, void* out_lo, int32_t* overflow, void* stream);
 
 /* Dense NHWC convolution on planes [batch, h_in, w_in, c_in] through TMA tensor maps: 3x3 (stride 1 or 2) or 1x1
  * with zero padding `pad` (<= ksize / 2 + 1), or ksize == stride == s for s in {2, 3, 4} with pad 0 (the Conv2d

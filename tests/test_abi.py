@@ -27,9 +27,39 @@ def test_binding_table_covers_the_header():
     assert sorted(_lib.SIGNATURES) == _declared_functions()
 
 
-def test_version_and_error_string():
+def _plane_writers():
+    """{entry point: (takes out_hi, takes an overflow pointer)} for every function of the header; a parameter counts
+    when it is named in the signature or is a field of a params struct the signature takes."""
+    text = open(os.path.join(ROOT, "include", "det3d_b200.h")).read()
+    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
+    structs = {}
+    for body, name in re.findall(r"typedef\s+struct\s*\{(.*?)\}\s*(\w+)\s*;", text, flags=re.S):
+        structs[name] = set(re.findall(r"\b(\w+)\s*(?:\[[^\]]*\])?\s*;", body))
+    text = re.sub(r"typedef\s+struct\s*\{.*?\}\s*\w+\s*;", "", text, flags=re.S)
+    out = {}
+    for name, args in re.findall(r"\b(d3b_[a-z0-9_]+)\s*\(([^;{]*?)\)\s*;", text, flags=re.S):
+        params = set(re.findall(r"\b(\w+)\s*(?:\[[^\]]*\])?\s*(?:,|$)", args.strip()))
+        for t in re.findall(r"\b(\w+)\s*\*", args):
+            params |= structs.get(t, set())
+        out[name] = ("out_hi" in params, "overflow" in params)
+    return out
+
+
+def test_every_plane_writer_takes_an_overflow_flag():
+    """A value that leaves the f16 range cannot be carried by the hi / lo planes, so every entry point that writes planes
+    (`out_hi`, as a parameter or a field of its params struct) must take the device flag that reports it."""
+    writers = _plane_writers()
+    assert len(writers) == len(_declared_functions())
+    planes = {n for n, (hi, _) in writers.items() if hi}
+    assert {"d3b_sparse_conv16", "d3b_bev_conv16", "d3b_sparse_to_bev16"} <= planes
+    missing = sorted(n for n in planes if not writers[n][1])
+    assert not missing, "write f16 planes without an overflow flag: %s" % missing
+
+
+def test_abi_version_and_error_string():
+    """ABI 3: d3b_sparse_to_bev16 takes the f16-range `overflow` flag (one argument more than in ABI 2)."""
     L = _lib.lib()
-    assert L.d3b_abi_version() == 2
+    assert L.d3b_abi_version() == 3
     assert isinstance(L.d3b_last_error(), bytes)
     assert L.d3b_launch_count() >= 0
 

@@ -499,8 +499,9 @@ def test_dense_magnitude_sweep(a_exp, w_exp):
     check_against_model(got, ref, layer.w_exp, "dense 2^%d x 2^%d" % (a_exp, w_exp))
 
 
-BOUNDARY = [(65503.99, 0), (-65503.99, 0), (65504.0, 1), (-65504.0, 1), (1.0e5, 1), (float("inf"), 1),
-            (float("-inf"), 1), (float("nan"), 1), (1.0, 0)]
+# 65519.99 still rounds to a finite hi (65504), 65520 is the first value whose hi is inf: both must be flagged
+BOUNDARY = [(65503.99, 0), (-65503.99, 0), (65504.0, 1), (-65504.0, 1), (65519.99, 1), (-65519.99, 1), (65520.0, 1),
+            (-65520.0, 1), (1.0e5, 1), (float("inf"), 1), (float("-inf"), 1), (float("nan"), 1), (1.0, 0)]
 
 
 def test_overflow_flag_boundary():
