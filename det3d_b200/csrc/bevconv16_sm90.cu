@@ -479,6 +479,208 @@ bev_conv16_cs_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
   D3B_CTA_MARK(1, g.seq);
 }
 
+// ======================================================================================================================
+// Variant "pipelined" (3x3, stride 1, output blocks of 128 channels, C_in % 64 == 0, up = 1; the automatic choice):
+// tile = 16 rows x 8 columns x 128 channels (one half of the pixel-stationary tile).  Each consumer warpgroup owns one
+// wgmma M = 64 block (8 x 8 pixels) x N = 128, i.e. 64 fp32 sums per thread, and computes a slot's 12-MMA partial as
+// one m64n128k16 chain into one of two 64-register partials: slot s is issued into P[s & 1] while slot s - 1 is still
+// running, then `wait_group 1` and s - 1 is folded.  Sums + two partials fit the 232 registers the consumer warpgroups
+// take with setmaxnreg (the producer warpgroup keeps 40), so nothing spills and the tensor pipe always has the next slot
+// queued.  The small tile also balances the grid: SECOND's 200 x 176 plane is 286 tiles (3 rounds of 128 pixels on
+// 132 SMs) instead of 143 (2 rounds of 256).  Same products, same order, same fold, same correction and epilogue as
+// the pixel-stationary kernel: bit-identical to it.
+//  * A stage = one box per plane, 64 channels x 8 pixels x 18 rows (18 KB); block m reads kernel row ky at
+//    m * 8192 + ky * 1024.  B stage = [W_hi | W_lo] of one (kb, kx, ky).  Three stages of each.
+constexpr int kPlCout = 128;
+constexpr int kPlStages = 3;
+constexpr int kPlPatchBytes = (kBvTileY + 2) * kBvHalfX * 128;    // 18432
+constexpr int kPlAStageBytes = 2 * kPlPatchBytes;                 // hi, lo
+constexpr int kPlBBytes = 2 * kPlCout * 128;                      // [W_hi rows | W_lo rows]
+constexpr int kPlSmemBytes = kPlStages * (kPlAStageBytes + kPlBBytes) + 1024 + 256;
+constexpr int kPlConsumerRegs = 232, kPlProducerRegs = 40;        // 2 * 232 + 40 <= 512 per thread triple
+static_assert(2 * kPlConsumerRegs + kPlProducerRegs <= 512, "register budget of one SM");
+
+__global__ void __launch_bounds__(kBvThreads, 1)
+bev_conv16_pl_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, BvGeom g,
+                     const __half* __restrict__ packed, BvEpi epi, __half* __restrict__ out_hi,
+                     __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t a_base = smem_base;
+  const uint32_t b_base = a_base + kPlStages * kPlAStageBytes;
+  const uint32_t bar_base = b_base + kPlStages * kPlBBytes;
+  auto a_full = [&](uint32_t s) { return bar_base + 8u * s; };
+  auto a_empty = [&](uint32_t s) { return bar_base + 8u * (kPlStages + s); };
+  auto b_full = [&](uint32_t s) { return bar_base + 8u * (2 * kPlStages + s); };
+  auto b_empty = [&](uint32_t s) { return bar_base + 8u * (3 * kPlStages + s); };
+
+  D3B_CTA_MARK(0, g.seq);
+  pdl_launch_dependents();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tiles_per_group = g.batch * g.tiles_y * g.tiles_x;     // tiles_x counts 8-column tiles here
+  const int n_tiles = tiles_per_group * g.groups;
+  const int n_slots = 9 * g.n_kb;                                  // (kb, kx, ky), ky fastest
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kPlStages; ++s) {
+      mbar_init(a_full(s), 1); mbar_init(a_empty(s), kBvMathWarps);
+      mbar_init(b_full(s), 1); mbar_init(b_empty(s), kBvMathWarps);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    tma_prefetch_desc(&tm_hi);
+    tma_prefetch_desc(&tm_lo);
+  }
+  __syncthreads();
+  pdl_wait_prior_grid();             // everything below reads the previous layer's planes or writes buffers it may still read
+
+  auto decode = [&](int tile, int& grp, int& b, int& y0, int& x0) {
+    grp = tile / tiles_per_group;
+    int t = tile - grp * tiles_per_group;
+    b = t / (g.tiles_y * g.tiles_x);
+    t -= b * g.tiles_y * g.tiles_x;
+    y0 = (t / g.tiles_x) * kBvTileY;
+    x0 = (t % g.tiles_x) * kBvHalfX;
+  };
+
+  if (warp >= kBvTmaWarp) {
+    // ===================== TMA producer (one elected lane) =====================
+    regs_dealloc<kPlProducerRegs>();
+    if (warp == kBvTmaWarp && lane == 0) {
+      uint32_t a_it = 0, b_it = 0;
+      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        int grp, b, y0, x0;
+        decode(tile, grp, b, y0, x0);
+        const __half* wgrp = packed + (size_t)grp * 9 * g.n_kb * (kPlBBytes / 2);
+        for (int kb = 0; kb < g.n_kb; ++kb) {
+          for (int kx = 0; kx < 3; ++kx, ++a_it) {
+            const uint32_t sa = a_it % kPlStages;
+            D3B_WAIT(a_empty(sa), ((a_it / kPlStages) & 1u) ^ 1u, 1);
+            mbar_arrive_expect_tx(a_full(sa), kPlAStageBytes);
+            const uint32_t dst = a_base + sa * kPlAStageBytes;
+            tma_load_4d(dst, &tm_hi, kb * kBvKc, x0 + kx - g.pad, y0 - g.pad, b, a_full(sa));
+            tma_load_4d(dst + kPlPatchBytes, &tm_lo, kb * kBvKc, x0 + kx - g.pad, y0 - g.pad, b, a_full(sa));
+            for (int ky = 0; ky < 3; ++ky, ++b_it) {
+              const uint32_t sb = b_it % kPlStages;
+              D3B_WAIT(b_empty(sb), ((b_it / kPlStages) & 1u) ^ 1u, 2);
+              mbar_arrive_expect_tx(b_full(sb), kPlBBytes);
+              tma_bulk_g2s(b_base + sb * kPlBBytes, wgrp + ((size_t)(ky * 3 + kx) * g.n_kb + kb) * (kPlBBytes / 2),
+                           kPlBBytes, b_full(sb));
+            }
+          }
+        }
+      }
+    }
+  } else {
+    // ===================== consumer warpgroups: warpgroup m -> tile rows [8m, 8m + 8) =====================
+    regs_alloc<kPlConsumerRegs>();
+    const int m = warp >> 2, wq = warp & 3;
+    bool ovf = false;
+    uint32_t a_it = 0, b_it = 0;                 // ring positions of the tile's first A / B stage
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+      int grp, b, y0, x0;
+      decode(tile, grp, b, y0, x0);
+      float acc[kPlCout / 2], p0[kPlCout / 2], p1[kPlCout / 2];
+#pragma unroll
+      for (int q = 0; q < kPlCout / 2; ++q) acc[q] = 0.f;
+      // slot s = (kb, kx, ky): its 12 MMAs into the partial P, committed as one group
+      auto issue = [&](float (&P)[kPlCout / 2], int s) {
+        const int ky = s % 3;
+        const uint32_t ai = a_it + s / 3, bi = b_it + s;
+        const uint32_t sa = ai % kPlStages, sb = bi % kPlStages;
+        if (ky == 0) D3B_WAIT(a_full(sa), (ai / kPlStages) & 1u, 4);
+        D3B_WAIT(b_full(sb), (bi / kPlStages) & 1u, 5);
+        const uint32_t a_hi = a_base + sa * kPlAStageBytes + m * 8192u + (uint32_t)ky * 1024u, a_lo = a_hi + kPlPatchBytes;
+        const uint32_t b_hi = b_base + sb * kPlBBytes, b_lo = b_hi + kPlCout * 128;
+        gmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < kBvKc / 16; ++ks) {
+          const uint32_t adv = ks * 32;
+          // small terms first, the dominant hi.hi product last (the order of the pixel-stationary kernel)
+          wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_lo + adv), gmma_desc_sw128(b_hi + adv), ks > 0 ? 1u : 0u);
+          wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_lo + adv), 1u);
+          wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + adv), 1u);
+        }
+        gmma_commit();
+      };
+      // slot s has completed: fold its partial (round-to-nearest) and release its stages
+      auto retire = [&](float (&P)[kPlCout / 2], int s) {
+        gmma_fence_regs(P);
+#pragma unroll
+        for (int q = 0; q < kPlCout / 2; ++q) acc[q] += P[q];
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(b_empty((b_it + s) % kPlStages));
+          if (s % 3 == 2) mbar_arrive(a_empty((a_it + s / 3) % kPlStages));
+        }
+      };
+      for (int s = 0; s < n_slots; s += 2) {
+        issue(p0, s);
+        if (s > 0) {
+          gmma_wait_pending<1>();
+          retire(p1, s - 1);
+        }
+        if (s + 1 < n_slots) {
+          issue(p1, s + 1);
+          gmma_wait_pending<1>();
+          retire(p0, s);
+        }
+      }
+      gmma_wait();
+      if (n_slots & 1) retire(p0, n_slots - 1);
+      else retire(p1, n_slots - 1);
+      a_it += n_slots / 3;
+      b_it += n_slots;
+
+      // epilogue, column block outer: each column pair's parameters are loaded once and used for both rows of the
+      // thread (row outer keeps all 16 blocks' parameters live next to the sums and spills)
+      const int cg = grp % g.cgroups;
+      const int pcol = grp * kPlCout;           // per-group epilogue parameters are laid out group-major
+      const int x = x0 + (lane >> 2);
+      bool live[2];
+      size_t row_off[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int y = y0 + 8 * m + 2 * wq + h;
+        live[h] = y < g.h_out && x < g.w_out;
+        row_off[h] = (((size_t)b * g.out_h + y) * g.out_w + x) * (size_t)g.out_channels + g.out_c0 + cg * kPlCout;
+      }
+#pragma unroll
+      for (int jn = 0; jn < kPlCout / 8; ++jn) {
+        const int col = jn * 8 + 2 * (lane & 3);
+        float2 bb, sc, sh;
+        if (epi.bias) bb = __ldg(reinterpret_cast<const float2*>(epi.bias + pcol + col));
+        if (epi.scale) {
+          sc = __ldg(reinterpret_cast<const float2*>(epi.scale + pcol + col));
+          sh = __ldg(reinterpret_cast<const float2*>(epi.shift + pcol + col));
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!live[h]) continue;
+          float v0 = acc[4 * jn + 2 * h] * epi.acc_scale, v1 = acc[4 * jn + 2 * h + 1] * epi.acc_scale;
+          v0 = fmaf(v0, epi.corr, v0);
+          v1 = fmaf(v1, epi.corr, v1);
+          if (epi.bias) { v0 += bb.x; v1 += bb.y; }
+          if (epi.scale) { v0 = fmaf(v0, sc.x, sh.x); v1 = fmaf(v1, sc.y, sh.y); }
+          if (epi.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+          if (out_hi) {
+            __half h0, l0, h1, l1;
+            split_f16(v0, h0, l0);
+            split_f16(v1, h1, l1);
+            *reinterpret_cast<uint32_t*>(out_hi + row_off[h] + col) = bv_pack_half2(h0, h1);
+            *reinterpret_cast<uint32_t*>(out_lo + row_off[h] + col) = bv_pack_half2(l0, l1);
+            ovf |= !(fabsf(v0) < 65504.f) | !(fabsf(v1) < 65504.f);
+          }
+          if (out_f32) *reinterpret_cast<float2*>(out_f32 + row_off[h] + col) = make_float2(v0, v1);
+        }
+      }
+      // one flag write per thread, after its last tile (placed after the tile loop, it costs 40 registers: ptxas
+      // then spills the sums)
+      if (tile + (int)gridDim.x >= n_tiles && ovf && overflow) atomicOr(overflow, 1);
+    }
+  }
+  D3B_CTA_MARK(1, g.seq);
+}
+
 // ---- host side: tensor maps through the driver entry point (libcuda is not linked: CPU hosts must dlopen us) ----------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -563,6 +765,28 @@ static int launch_bev_cs(const d3b_bev16_params* p, const BvGeom& g, cudaStream_
   return D3B_OK;
 }
 
+// pipelined variant: 3x3, stride 1, output blocks of 128 channels, C_in % 64 == 0, no sub-pixel groups
+static int launch_bev_pl(const d3b_bev16_params* p, BvGeom g, cudaStream_t stream) {
+  static SmemOptIn optin;
+  D3B_CUDA(ensure_dynamic_smem(bev_conv16_pl_kernel, kPlSmemBytes, optin));
+  CUtensorMap tm_hi, tm_lo;
+  int st = make_map(&tm_hi, p->in_hi, p->batch, p->h_in, p->w_in, p->c_in, kBvHalfX, kBvTileY + 2, 1);
+  if (st != D3B_OK) return st;
+  st = make_map(&tm_lo, p->in_lo, p->batch, p->h_in, p->w_in, p->c_in, kBvHalfX, kBvTileY + 2, 1);
+  if (st != D3B_OK) return st;
+  BvEpi e;
+  e.bias = p->bias; e.scale = p->scale; e.shift = p->shift; e.acc_scale = p->acc_scale; e.relu = p->relu;
+  e.corr = trunc_correction(p->c_in);
+  g.tiles_x = div_up(g.w_out, kBvHalfX);     // tiles of 16 rows x 8 columns
+  const int n_tiles = g.batch * g.tiles_y * g.tiles_x * g.groups;
+  const int grid = n_tiles < kNumSMs ? n_tiles : kNumSMs;
+  D3B_CUDA(launch_maybe_pdl(bev_conv16_pl_kernel, dim3(grid), dim3(kBvThreads), kPlSmemBytes, stream, tm_hi, tm_lo, g,
+                            (const __half*)p->weight_packed, e, (__half*)p->out_hi, (__half*)p->out_lo, p->out_f32,
+                            (int*)p->overflow));
+  D3B_LAUNCH_CHECK();
+  return D3B_OK;
+}
+
 }  // namespace d3b
 
 using namespace d3b;
@@ -605,13 +829,13 @@ extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
   g.out_channels = p->out_channels; g.out_c0 = p->out_c0;
   static std::atomic<int> launch_seq{0};
   g.seq = launch_seq.fetch_add(1, std::memory_order_relaxed);
-  // Automatic (variant 2) = pixel-stationary: on the H100 it is the faster schedule (H100 80GB HBM3 at a 700 W limit,
-  // PointPillars, B = 1, 20k points: dense 3x3 layers 4.0 ms/step pixel-stationary vs 5.4 ms channel-stationary; CBGS,
-  // whose launches have fewer tiles than SMs, measured the same either way).  The channel-stationary kernel stays selectable (variant 1) and gives the same bits.
+  // Automatic (variant 2) = the pipelined kernel for the 3x3 stride-1 layers with 128-channel output blocks, the
+  // pixel-stationary kernel for every other shape.  Variant 0 (pixel-stationary everywhere) is the reference the other
+  // two reproduce bit for bit; variant 1 selects the channel-stationary kernel for the 3x3 stride-1 layers.
   const int variant = bev_variant();
-  if (variant == 1 && p->ksize == 3 && p->stride == 1 && p->c_out == kBwCout &&
-      p->c_in % kBvKc == 0 && p->up == 1 && p->out_channels % 4 == 0)
-    return launch_bev_cs(p, g, stream);
+  const bool s1_blocks = p->ksize == 3 && p->stride == 1 && p->c_out == kBwCout && p->c_in % kBvKc == 0 && p->up == 1;
+  if (variant == 1 && s1_blocks && p->out_channels % 4 == 0) return launch_bev_cs(p, g, stream);
+  if (variant == 2 && s1_blocks) return launch_bev_pl(p, g, stream);
 #define D3B_BEV_CASE(KS, ST)                                                   \
   if (p->ksize == KS && p->stride == ST) {                                     \
     switch (p->c_out) {                                                        \

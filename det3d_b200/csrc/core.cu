@@ -22,7 +22,7 @@ static std::atomic<int> g_pdl{1};
 bool pdl_enabled() { return g_pdl.load(std::memory_order_relaxed) != 0; }
 
 // default schedule of the 3x3 stride-1 dense layers; the environment variable D3B_BEV_VARIANT overrides it at load
-constexpr int kDefaultBevVariant = 2;      // automatic (pixel-stationary): see d3b_set_bev_variant
+constexpr int kDefaultBevVariant = 2;      // automatic (pipelined 3x3 stride-1 kernel): see d3b_set_bev_variant
 static int initial_bev_variant() {
   const char* e = std::getenv("D3B_BEV_VARIANT");
   if (e != nullptr && e[0] >= '0' && e[0] <= '2' && e[1] == 0) return e[0] - '0';

@@ -258,6 +258,14 @@ __device__ __forceinline__ void gmma_fence() { asm volatile("wgmma.fence.sync.al
 __device__ __forceinline__ void gmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 // waits for every committed wgmma of this warpgroup: its operands have been read and its accumulators are final
 __device__ __forceinline__ void gmma_wait() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// waits until at most N committed wgmma groups of this warpgroup are still in flight
+template <int N>
+__device__ __forceinline__ void gmma_wait_pending() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// per-warpgroup register budget (warp-specialised kernels): the producer gives registers back, the consumers take them
+template <int R>
+__device__ __forceinline__ void regs_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void regs_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 // keeps the compiler from moving accumulator accesses across the asynchronous MMAs
 template <int R>
 __device__ __forceinline__ void gmma_fence_regs(float (&d)[R]) {
