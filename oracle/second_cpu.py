@@ -115,11 +115,12 @@ class SecondCPU:
             nums.append(n)
         return np.concatenate(vox), np.concatenate(coors), np.concatenate(nums)
 
-    def backbone(self, voxels, coors, nums, batch):
+    def backbone(self, voxels, coors, nums, batch, **kw):
+        """Reader (per-voxel mean, fp32) + middle encoder; `kw` goes to middle_encoder_forward (dtype, return_levels)."""
         feats = torch.from_numpy(voxels[:, :, : self.cfg.model["reader"]["num_input_features"]]).sum(1) / \
             torch.from_numpy(nums).float().view(-1, 1)
         sd = {k[len("backbone."):]: v for k, v in self.sd.items() if k.startswith("backbone.")}
-        return ospconv.middle_encoder_forward(sd, feats, coors, batch, [int(g) for g in self.grid], arch=self.arch)
+        return ospconv.middle_encoder_forward(sd, feats, coors, batch, [int(g) for g in self.grid], arch=self.arch, **kw)
 
     def head(self, x):
         t = "bbox_head.tasks.0."

@@ -115,12 +115,12 @@ def pairs_of(nbr):
     return trip[np.lexsort((trip[:, 2], trip[:, 1], trip[:, 0]))]
 
 
-def indice_conv(features, weight, nbr, n_out, bias=None):
-    """spconv v1 indice_conv: for every offset with pairs, gather -> mm -> scatter-add (fp32)."""
-    feats = torch.as_tensor(features, dtype=torch.float32)
-    w = torch.as_tensor(weight, dtype=torch.float32)
+def indice_conv(features, weight, nbr, n_out, bias=None, dtype=torch.float32):
+    """spconv v1 indice_conv: for every offset with pairs, gather -> mm -> scatter-add (in `dtype`, fp32 by default)."""
+    feats = torch.as_tensor(features, dtype=dtype)
+    w = torch.as_tensor(weight, dtype=dtype)
     w = w.reshape(-1, w.shape[-2], w.shape[-1])
-    out = torch.zeros((n_out, w.shape[2]), dtype=torch.float32)
+    out = torch.zeros((n_out, w.shape[2]), dtype=dtype)
     for k in range(w.shape[0]):
         o = np.nonzero(nbr[k] >= 0)[0]
         if o.size == 0:
@@ -128,15 +128,15 @@ def indice_conv(features, weight, nbr, n_out, bias=None):
         i = torch.from_numpy(nbr[k][o])
         out.index_add_(0, torch.from_numpy(o), feats[i] @ w[k])
     if bias is not None:
-        out += torch.as_tensor(bias, dtype=torch.float32)
+        out += torch.as_tensor(bias, dtype=dtype)
     return out
 
 
-def dense(features, coors, spatial, batch):
-    feats = torch.as_tensor(features, dtype=torch.float32)
+def dense(features, coors, spatial, batch, dtype=torch.float32):
+    feats = torch.as_tensor(features, dtype=dtype)
     c = torch.as_tensor(np.asarray(coors)).long()
     d, h, w = spatial
-    out = torch.zeros((batch, d, h, w, feats.shape[1]), dtype=torch.float32)
+    out = torch.zeros((batch, d, h, w, feats.shape[1]), dtype=dtype)
     out[c[:, 0], c[:, 1], c[:, 2], c[:, 3]] = feats
     return out.permute(0, 4, 1, 2, 3).contiguous()
 
@@ -193,27 +193,36 @@ def _spec_fhd(cin):
 
 
 def middle_encoder_forward(state_dict, voxel_features, coors, batch_size, input_shape, arch="SpMiddleFHD",
-                           eps=1e-3, return_levels=False):
-    """CPU forward of SpMiddleFHD / SpMiddleResNetFHD from a `middle_conv.*` state_dict.
+                           eps=1e-3, return_levels=False, dtype=torch.float32):
+    """CPU forward of SpMiddleFHD / SpMiddleResNetFHD from a `middle_conv.*` state_dict, in `dtype` (fp32 by default;
+    float64 gives a reference the fp32 device encoder can be measured against).
 
     Mirrors scn.py:184-197 / :357-370: sparse_shape = input_shape[::-1] + [1,0,0], the
     SparseSequential, .dense(), view(N, C*D, H, W).
+
+    With return_levels=True, also returns one record per conv layer, in execution order: kind ("subm" / "conv"), the
+    state_dict prefixes of its conv and BatchNorm, nbr [K, N_out] and the output coors / spatial shape, and the values
+    around it -- `input` (the features it convolves), `identity` (the block input a residual layer adds before its ReLU,
+    else None) and `output` (after BatchNorm, residual and ReLU: the next layer's input).
     """
-    sd = {k: torch.as_tensor(v).float() if torch.is_tensor(v) or isinstance(v, np.ndarray) else v
+    sd = {k: torch.as_tensor(v).to(dtype) if torch.is_tensor(v) or isinstance(v, np.ndarray) else v
           for k, v in state_dict.items()}
     spatial = tuple(int(s) for s in (np.array(input_shape[::-1]) + [1, 0, 0]))
     coors = np.asarray(coors).astype(np.int32)
-    x = torch.as_tensor(voxel_features, dtype=torch.float32)
+    x = torch.as_tensor(voxel_features, dtype=dtype)
     cache = {}
     levels = []
 
     def bn(prefix, t):
+        levels[-1]["bn"] = prefix
         return batchnorm_eval(t, dict(running_mean=sd[prefix + ".running_mean"], running_var=sd[prefix + ".running_var"],
                                       weight=sd[prefix + ".weight"], bias=sd[prefix + ".bias"], eps=eps))
 
     def conv(prefix, t, cur_coors, cur_sp, kind, k, s, p, key):
         w = sd[prefix + ".weight"]
         b = sd.get(prefix + ".bias")
+        rec = dict(kind=kind, conv=prefix, bn=None, input=t, identity=None, output=None)
+        levels.append(rec)
         if kind == "subm":
             ck = (key, cur_sp, cur_coors.shape[0])
             if key is None or ck not in cache:
@@ -222,34 +231,39 @@ def middle_encoder_forward(state_dict, voxel_features, coors, batch_size, input_
                     cache[ck] = nbr
             else:
                 nbr = cache[ck]
-            levels.append(dict(kind=kind, nbr=nbr, coors=cur_coors, spatial=cur_sp))
-            return indice_conv(t, w, nbr, cur_coors.shape[0], b), cur_coors, cur_sp
+            rec.update(nbr=nbr, coors=cur_coors, spatial=cur_sp)
+            return indice_conv(t, w, nbr, cur_coors.shape[0], b, dtype), cur_coors, cur_sp
         oc, osp = conv_outputs(cur_coors, cur_sp, k, s, p)
         nbr = conv_neighbours(cur_coors, cur_sp, oc, k, s, p)
-        levels.append(dict(kind=kind, nbr=nbr, coors=oc, spatial=osp))
-        return indice_conv(t, w, nbr, oc.shape[0], b), oc, osp
+        rec.update(nbr=nbr, coors=oc, spatial=osp)
+        return indice_conv(t, w, nbr, oc.shape[0], b, dtype), oc, osp
+
+    def done(t):
+        levels[-1]["output"] = t
+        return t
 
     cur_coors, cur_sp = coors, spatial
     if arch == "SpMiddleFHD":
         idx = 0
         for (kind, ci, co, k, s, p, key) in _spec_fhd(x.shape[1]):
             x, cur_coors, cur_sp = conv("middle_conv.%d" % idx, x, cur_coors, cur_sp, kind, k, s, p, key)
-            x = torch.relu(bn("middle_conv.%d" % (idx + 1), x))
+            x = done(torch.relu(bn("middle_conv.%d" % (idx + 1), x)))
             idx += 3
     elif arch == "SpMiddleResNetFHD":
         def block(i, t, key):
             pre = "middle_conv.%d" % i
             idt = t
             o, _, _ = conv(pre + ".conv1", t, cur_coors, cur_sp, "subm", 3, None, None, key)
-            o = torch.relu(bn(pre + ".bn1", o))
+            o = done(torch.relu(bn(pre + ".bn1", o)))
             o, _, _ = conv(pre + ".conv2", o, cur_coors, cur_sp, "subm", 3, None, None, key)
+            levels[-1]["identity"] = idt
             o = bn(pre + ".bn2", o)
-            return torch.relu(o + idt)
+            return done(torch.relu(o + idt))
 
         def stem(i, t, kind, k, s, p, key):
             nonlocal cur_coors, cur_sp
             t, cur_coors, cur_sp = conv("middle_conv.%d" % i, t, cur_coors, cur_sp, kind, k, s, p, key)
-            return torch.relu(bn("middle_conv.%d" % (i + 1), t))
+            return done(torch.relu(bn("middle_conv.%d" % (i + 1), t)))
 
         x = stem(0, x, "subm", 3, None, None, "res0")
         x = block(3, x, "res0"); x = block(4, x, "res0")
@@ -262,7 +276,7 @@ def middle_encoder_forward(state_dict, voxel_features, coors, batch_size, input_
         x = stem(20, x, "conv", (3, 1, 1), (2, 1, 1), 0, None)
     else:
         raise ValueError(arch)
-    out = dense(x, cur_coors, cur_sp, batch_size)
+    out = dense(x, cur_coors, cur_sp, batch_size, dtype)
     n, c, d, h, w = out.shape
     out = out.view(n, c * d, h, w)
     if return_levels:

@@ -212,8 +212,8 @@ def test_cbgs_nuscenes_config():
     ConvTranspose deblock, 6 task heads, 9-dim boxes with angle-vector encoding), 35k-point 5-feature clouds, 4 clouds
     per GPU as in the 32-over-8 sharding.  RPN + heads run on the FP16x3 TMA kernels and are checked against the module's
     fp32 cuDNN forward; the device predict is checked against the CPU restatement of MultiGroupHead.predict on the same
-    head outputs: identical detections.  (The sparse encoder is pinned against the oracle in test_spconv_gpu; the
-    32-cloud multi-GPU run in test_multi_gpu.)"""
+    head outputs: identical detections.  (The sparse encoder at this shape is pinned against the float64 oracle, stage by
+    stage and layer by layer, in test_encoder_deployed_gpu; the 32-cloud multi-GPU run in test_multi_gpu.)"""
     from det3d.models import build_detector
     from det3d.torchie import Config
     from det3d_b200.apis import InferencePipeline
