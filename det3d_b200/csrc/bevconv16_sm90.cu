@@ -32,18 +32,9 @@
 // executes 3x that.  Algorithmic bytes = B*H*W*(C_in + C_out)*4 + K*K*C_in*C_out*4.
 #include <cuda.h>
 
-#include "gmma.cuh"
+#include "epilogue16.cuh"
 
 namespace d3b {
-
-struct BvEpi {          // same fields as spconv16_sm90.cu (kept local: the two kernels are separate TUs)
-  const float* bias;
-  const float* scale;
-  const float* shift;
-  float acc_scale;
-  float corr;           // mean truncation of the layer's partials (gmma.cuh), applied to the sums
-  int relu;
-};
 
 constexpr int kBvTileY = 16, kBvTileX = 16;     // output pixels per tile
 constexpr int kBvHalfX = 8;                     // one half = 16 rows x 8 columns = two wgmma M = 64 blocks
@@ -76,18 +67,12 @@ struct BvGeom {
   int up;                         // output pixel = (y*up + uy, x*up + ux)
   int out_h, out_w;               // output tensor grid (h_out*up, w_out*up)
   int out_channels, out_c0;       // row length of the output tensor and first channel written
-  int seq;                        // launch counter of this translation unit (development traces only)
 };
-
-__device__ __forceinline__ uint32_t bv_pack_half2(__half a, __half b) {
-  return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
-}
-
 
 template <int KS, int STRIDE, int COUT>
 __global__ void __launch_bounds__(kBvThreads, 1)
 bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, BvGeom g,
-                  const __half* __restrict__ packed, BvEpi epi, __half* __restrict__ out_hi,
+                  const __half* __restrict__ packed, Epi16 epi, __half* __restrict__ out_hi,
                   __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
   using Cfg = BvCfg<KS, STRIDE, COUT>;
   extern __shared__ uint8_t smem_raw[];
@@ -100,7 +85,7 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
   auto b_full = [&](int s) { return bar_base + 8u * (2 * kBvAStages + s); };
   auto b_empty = [&](int s) { return bar_base + 8u * (2 * kBvAStages + Cfg::kBStages + s); };
 
-  D3B_CTA_MARK(0, g.seq);
+  D3B_CTA_MARK(0, epi.seq);
   pdl_launch_dependents();           // the next kernel of the stream may start its prologue behind this one's tail
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_group = g.batch * g.tiles_y * g.tiles_x;
@@ -261,12 +246,10 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
             }
             if (epi.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
             if (out_hi) {
-              __half h0, l0, h1, l1;
-              split_f16(v0, h0, l0);
-              split_f16(v1, h1, l1);
-              *reinterpret_cast<uint32_t*>(out_hi + row_off + col) = bv_pack_half2(h0, h1);
-              *reinterpret_cast<uint32_t*>(out_lo + row_off + col) = bv_pack_half2(l0, l1);
-              ovf |= !(fabsf(v0) < 65504.f) | !(fabsf(v1) < 65504.f);
+              uint32_t hi, lo;
+              ovf |= split_pack2(v0, v1, hi, lo);
+              *reinterpret_cast<uint32_t*>(out_hi + row_off + col) = hi;
+              *reinterpret_cast<uint32_t*>(out_lo + row_off + col) = lo;
             }
             if (out_f32) *reinterpret_cast<float2*>(out_f32 + row_off + col) = make_float2(v0, v1);
           }
@@ -275,208 +258,7 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
     }
     if (ovf && overflow) atomicOr(overflow, 1);
   }
-  D3B_CTA_MARK(1, g.seq);
-}
-
-// ======================================================================================================================
-// Variant "channel-stationary" (3x3, stride 1, C_out = 128 per group, C_in % 64 == 0, up = 1): the GEMM is transposed,
-//     D^T[C_out = 128 (M), 256 pixels (N)] += W[C_out, K16] . Act[256 pixels, K16]^T
-// so each consumer warpgroup covers 64 channels of the 16 x 16 pixel tile in four N = 64 column passes: the weights
-// are the A operand and pixels the N dimension.  Same products, same order, same partials and truncation correction as
-// the pixel-stationary kernel.
-//  * Activations: one TMA box per plane = 64 channels x 16 pixels x 18 rows: an image row is 2048 B (two swizzle groups),
-//    pixel (r, x) of the tile is operand row r * 16 + x, kernel row ky = descriptor start + ky * 2048.
-//  * Weights: the packed [W_hi | W_lo] image is K-major SW128 with C_out rows -- byte for byte usable as the A operand.
-//  * Accumulators: a thread holds 2 channels x 64 pixels, so bias / BN parameters are per-thread scalars.
-constexpr int kBwThreads = 384;                                   // warps 0..7 consumers, 8 activation TMA, 9 weights, 10..11 idle
-constexpr int kBwActWarp = 8;
-constexpr int kBwWeightWarp = 9;
-constexpr int kBwCout = 128;
-constexpr int kBwPatchRows = kBvTileY + 2;                        // 18
-constexpr int kBwRowBytes = kBvTileX * 128;                       // one image row of the patch: 16 pixels x 128 B
-constexpr int kBwPatchBytes = kBwPatchRows * kBwRowBytes;         // 36864
-constexpr int kBwAStageBytes = 2 * kBwPatchBytes;                 // hi, lo
-constexpr int kBwBBytes = 2 * kBwCout * 128;                      // [W_hi rows | W_lo rows]
-constexpr int kBwBStages = 2;
-constexpr int kBwPixels = kBvTileY * kBvTileX;                    // 256 pixel columns per tile
-constexpr int kBwSmemBytes = kBvAStages * kBwAStageBytes + kBwBStages * kBwBBytes + 1024 + 256;
-
-__global__ void __launch_bounds__(kBwThreads, 1)
-bev_conv16_cs_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, BvGeom g,
-                     const __half* __restrict__ packed, BvEpi epi, __half* __restrict__ out_hi,
-                     __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t a_base = smem_base;
-  const uint32_t b_base = a_base + kBvAStages * kBwAStageBytes;
-  const uint32_t bar_base = b_base + kBwBStages * kBwBBytes;
-  auto a_full = [&](int s) { return bar_base + 8u * s; };
-  auto a_empty = [&](int s) { return bar_base + 8u * (2 + s); };
-  auto b_full = [&](int s) { return bar_base + 8u * (4 + s); };
-  auto b_empty = [&](int s) { return bar_base + 8u * (6 + s); };
-
-  D3B_CTA_MARK(0, g.seq);
-  pdl_launch_dependents();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tiles_per_group = g.batch * g.tiles_y * g.tiles_x;
-  const int n_tiles = tiles_per_group * g.groups;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(a_full(s), 1); mbar_init(a_empty(s), kBvMathWarps);
-      mbar_init(b_full(s), 1); mbar_init(b_empty(s), kBvMathWarps);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    tma_prefetch_desc(&tm_hi);
-    tma_prefetch_desc(&tm_lo);
-  }
-  __syncthreads();
-  // (griddepcontrol.wait is executed by the threads that touch the previous layer's planes or write outputs: the activation
-  // producer and the consumers; weight staging runs ahead of the previous grid's tail)
-
-  auto decode = [&](int tile, int& grp, int& b, int& y0, int& x0) {
-    grp = tile / tiles_per_group;
-    int t = tile - grp * tiles_per_group;
-    b = t / (g.tiles_y * g.tiles_x);
-    t -= b * g.tiles_y * g.tiles_x;
-    y0 = (t / g.tiles_x) * kBvTileY;
-    x0 = (t % g.tiles_x) * kBvTileX;
-  };
-
-  if (warp == kBwActWarp) {
-    // ===================== activation producer (TMA tensor loads) =====================
-    // (Weights have their own producer warp: with one thread feeding both rings, the next patch load would queue up
-    // behind a wait for a free weight stage.)
-    if (lane == 0) {
-      pdl_wait_prior_grid();           // the planes are the previous layer's output
-      uint32_t a_it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        int grp, b, y0, x0;
-        decode(tile, grp, b, y0, x0);
-        for (int kb = 0; kb < g.n_kb; ++kb) {
-          for (int kx = 0; kx < 3; ++kx, ++a_it) {
-            const int sa = a_it & 1;
-            D3B_STAMP(0, a_it);
-            D3B_WAIT(a_empty(sa), ((a_it >> 1) & 1u) ^ 1u, 1);
-            mbar_arrive_expect_tx(a_full(sa), kBwAStageBytes);
-            const uint32_t dst = a_base + sa * kBwAStageBytes;
-            tma_load_4d(dst, &tm_hi, kb * kBvKc, x0 + kx - g.pad, y0 - g.pad, b, a_full(sa));
-            tma_load_4d(dst + kBwPatchBytes, &tm_lo, kb * kBvKc, x0 + kx - g.pad, y0 - g.pad, b, a_full(sa));
-            D3B_STAMP(1, a_it);
-          }
-        }
-      }
-    }
-  } else if (warp == kBwWeightWarp) {
-    // ===================== weight producer (bulk copies; weights do not depend on the previous grid) =====================
-    if (lane == 0) {
-      uint32_t b_it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int grp = tile / tiles_per_group;
-        const __half* wgrp = packed + (size_t)grp * 9 * g.n_kb * (kBwBBytes / 2);
-        for (int kb = 0; kb < g.n_kb; ++kb) {
-          for (int kx = 0; kx < 3; ++kx) {
-            for (int ky = 0; ky < 3; ++ky, ++b_it) {
-              const int sb = b_it & 1;
-              D3B_STAMP(2, b_it);
-              D3B_WAIT(b_empty(sb), ((b_it >> 1) & 1u) ^ 1u, 2);
-              mbar_arrive_expect_tx(b_full(sb), kBwBBytes);
-              tma_bulk_g2s(b_base + sb * kBwBBytes, wgrp + ((size_t)(ky * 3 + kx) * g.n_kb + kb) * (kBwBBytes / 2),
-                           kBwBBytes, b_full(sb));
-              D3B_STAMP(3, b_it);
-            }
-          }
-        }
-      }
-    }
-  } else if (warp < kBvMathWarps) {
-    // ===================== consumer warpgroups: warpgroup wg -> output channels [64 wg, 64 wg + 64) =====================
-    pdl_wait_prior_grid();                              // (output buffers may still be read by earlier kernels)
-    const int wg = warp >> 2, wq = warp & 3;
-    bool ovf = false;
-    uint32_t a_it = 0, b_it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      int grp, b, y0, x0;
-      decode(tile, grp, b, y0, x0);
-      float acc[kBwPixels / 2];
-#pragma unroll
-      for (int q = 0; q < kBwPixels / 2; ++q) acc[q] = 0.f;
-      for (int kb = 0; kb < g.n_kb; ++kb) {
-        for (int kx = 0; kx < 3; ++kx, ++a_it) {
-          const uint32_t sa = a_it & 1u;
-          if (warp == 0 && lane == 0) D3B_STAMP(4, a_it);
-          D3B_WAIT(a_full(sa), (a_it >> 1) & 1u, 4);
-          if (warp == 0 && lane == 0) D3B_STAMP(5, a_it);
-          for (int ky = 0; ky < 3; ++ky, ++b_it) {
-            const uint32_t sb = b_it & 1u;
-            D3B_WAIT(b_full(sb), (b_it >> 1) & 1u, 5);
-            if (warp == 0 && lane == 0) D3B_STAMP(6, b_it);
-            const uint32_t w_hi = b_base + sb * kBwBBytes + wg * 8192u, w_lo = w_hi + kBwCout * 128;
-            const uint32_t x_hi = a_base + sa * kBwAStageBytes + (uint32_t)ky * kBwRowBytes, x_lo = x_hi + kBwPatchBytes;
-#pragma unroll
-            for (int nh = 0; nh < 4; ++nh) {            // pixels [64 nh, 64 nh + 64): tile rows [4 nh, 4 nh + 4)
-              const uint32_t xo = nh * 64 * 128;
-              float part[32];
-              gmma_fence();
-#pragma unroll
-              for (int ks = 0; ks < kBvKc / 16; ++ks) {
-                const uint32_t adv = ks * 32;
-                // small terms first, the dominant hi.hi product last (the order of the pixel-stationary kernel)
-                wgmma_f16<64>(part, gmma_desc_sw128(w_hi + adv), gmma_desc_sw128(x_lo + xo + adv), ks > 0 ? 1u : 0u);
-                wgmma_f16<64>(part, gmma_desc_sw128(w_lo + adv), gmma_desc_sw128(x_hi + xo + adv), 1u);
-                wgmma_f16<64>(part, gmma_desc_sw128(w_hi + adv), gmma_desc_sw128(x_hi + xo + adv), 1u);
-              }
-              gmma_commit();
-              gmma_wait();
-              gmma_fence_regs(part);
-#pragma unroll
-              for (int q = 0; q < 32; ++q) acc[nh * 32 + q] += part[q];
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(b_empty(sb));
-            if (warp == 0 && lane == 0) D3B_STAMP(7, b_it);
-          }
-          if (lane == 0) mbar_arrive(a_empty(sa));
-        }
-      }
-      // ---- epilogue: per-channel scalars; a thread holds channels ch, ch + 8 of pixels 8 jn + 2 (lane % 4) + {0, 1} ----
-      const int cg = grp % g.cgroups;
-      const size_t chan0 = (size_t)g.out_c0 + (size_t)cg * kBwCout;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int ch = wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
-        const int pcol = grp * kBwCout + ch;
-        const float e_bias = epi.bias ? __ldg(epi.bias + pcol) : 0.f;
-        const float e_scale = epi.scale ? __ldg(epi.scale + pcol) : 1.f;
-        const float e_shift = epi.scale ? __ldg(epi.shift + pcol) : 0.f;
-#pragma unroll
-        for (int jn = 0; jn < kBwPixels / 8; ++jn) {
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            const int p = jn * 8 + 2 * (lane & 3) + c;
-            const int y = y0 + (p >> 4), x = x0 + (p & 15);
-            float v = acc[4 * jn + 2 * h + c] * epi.acc_scale;
-            v = fmaf(v, epi.corr, v);
-            if (epi.bias) v += e_bias;
-            if (epi.scale) v = fmaf(v, e_scale, e_shift);
-            if (epi.relu) v = fmaxf(v, 0.f);
-            if (!(y < g.h_out && x < g.w_out)) continue;
-            const size_t off = (((size_t)b * g.out_h + y) * g.out_w + x) * (size_t)g.out_channels + chan0 + ch;
-            if (out_hi) {
-              __half hh, ll;
-              split_f16(v, hh, ll);
-              out_hi[off] = hh;
-              out_lo[off] = ll;
-              ovf |= !(fabsf(v) < 65504.f);
-            }
-            if (out_f32) out_f32[off] = v;
-          }
-        }
-      }
-    }
-    if (ovf && overflow) atomicOr(overflow, 1);
-  }
-  D3B_CTA_MARK(1, g.seq);
+  D3B_CTA_MARK(1, epi.seq);
 }
 
 // ======================================================================================================================
@@ -502,7 +284,7 @@ static_assert(2 * kPlConsumerRegs + kPlProducerRegs <= 512, "register budget of 
 
 __global__ void __launch_bounds__(kBvThreads, 1)
 bev_conv16_pl_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, BvGeom g,
-                     const __half* __restrict__ packed, BvEpi epi, __half* __restrict__ out_hi,
+                     const __half* __restrict__ packed, Epi16 epi, __half* __restrict__ out_hi,
                      __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -514,7 +296,7 @@ bev_conv16_pl_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
   auto b_full = [&](uint32_t s) { return bar_base + 8u * (2 * kPlStages + s); };
   auto b_empty = [&](uint32_t s) { return bar_base + 8u * (3 * kPlStages + s); };
 
-  D3B_CTA_MARK(0, g.seq);
+  D3B_CTA_MARK(0, epi.seq);
   pdl_launch_dependents();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_group = g.batch * g.tiles_y * g.tiles_x;     // tiles_x counts 8-column tiles here
@@ -663,12 +445,10 @@ bev_conv16_pl_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
           if (epi.scale) { v0 = fmaf(v0, sc.x, sh.x); v1 = fmaf(v1, sc.y, sh.y); }
           if (epi.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
           if (out_hi) {
-            __half h0, l0, h1, l1;
-            split_f16(v0, h0, l0);
-            split_f16(v1, h1, l1);
-            *reinterpret_cast<uint32_t*>(out_hi + row_off[h] + col) = bv_pack_half2(h0, h1);
-            *reinterpret_cast<uint32_t*>(out_lo + row_off[h] + col) = bv_pack_half2(l0, l1);
-            ovf |= !(fabsf(v0) < 65504.f) | !(fabsf(v1) < 65504.f);
+            uint32_t hi, lo;
+            ovf |= split_pack2(v0, v1, hi, lo);
+            *reinterpret_cast<uint32_t*>(out_hi + row_off[h] + col) = hi;
+            *reinterpret_cast<uint32_t*>(out_lo + row_off[h] + col) = lo;
           }
           if (out_f32) *reinterpret_cast<float2*>(out_f32 + row_off[h] + col) = make_float2(v0, v1);
         }
@@ -678,7 +458,7 @@ bev_conv16_pl_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
       if (tile + (int)gridDim.x >= n_tiles && ovf && overflow) atomicOr(overflow, 1);
     }
   }
-  D3B_CTA_MARK(1, g.seq);
+  D3B_CTA_MARK(1, epi.seq);
 }
 
 // ---- host side: tensor maps through the driver entry point (libcuda is not linked: CPU hosts must dlopen us) ----------
@@ -722,45 +502,40 @@ static int make_map(CUtensorMap* map, const void* base, int batch, int h, int w,
   return D3B_OK;
 }
 
+// What both kernels are launched with: the tensor maps of the input planes (boxes of box_w pixels x box_h rows) and the
+// epilogue parameters.
+static int bev_args(const d3b_bev16_params* p, int box_w, int box_h, int stride, CUtensorMap* tm_hi, CUtensorMap* tm_lo,
+                    Epi16* e) {
+  int st = make_map(tm_hi, p->in_hi, p->batch, p->h_in, p->w_in, p->c_in, box_w, box_h, stride);
+  if (st == D3B_OK) st = make_map(tm_lo, p->in_lo, p->batch, p->h_in, p->w_in, p->c_in, box_w, box_h, stride);
+  if (st != D3B_OK) return st;
+  e->bias = p->bias; e->scale = p->scale; e->shift = p->shift;
+  e->res_hi = nullptr; e->res_lo = nullptr;
+  e->acc_scale = p->acc_scale; e->relu = p->relu;
+  e->corr = trunc_correction(p->c_in);
+  static std::atomic<int> launch_seq{0};
+  e->seq = launch_seq.fetch_add(1, std::memory_order_relaxed);
+  return D3B_OK;
+}
+
+// persistent grid: one CTA per tile, at most one per SM
+static int bev_grid(const BvGeom& g) {
+  const int n_tiles = g.batch * g.tiles_y * g.tiles_x * g.groups;
+  return n_tiles < kNumSMs ? n_tiles : kNumSMs;
+}
+
 template <int KS, int STRIDE, int COUT>
 static int launch_bev(const d3b_bev16_params* p, const BvGeom& g, cudaStream_t stream) {
   using Cfg = BvCfg<KS, STRIDE, COUT>;
   static SmemOptIn optin;
   D3B_CUDA(ensure_dynamic_smem(bev_conv16_kernel<KS, STRIDE, COUT>, Cfg::kSmemBytes, optin));
   CUtensorMap tm_hi, tm_lo;
-  int st = make_map(&tm_hi, p->in_hi, p->batch, p->h_in, p->w_in, p->c_in, kBvHalfX, Cfg::kPatchRows, STRIDE);
+  Epi16 e;
+  const int st = bev_args(p, kBvHalfX, Cfg::kPatchRows, STRIDE, &tm_hi, &tm_lo, &e);
   if (st != D3B_OK) return st;
-  st = make_map(&tm_lo, p->in_lo, p->batch, p->h_in, p->w_in, p->c_in, kBvHalfX, Cfg::kPatchRows, STRIDE);
-  if (st != D3B_OK) return st;
-  BvEpi e;
-  e.bias = p->bias; e.scale = p->scale; e.shift = p->shift; e.acc_scale = p->acc_scale; e.relu = p->relu;
-  e.corr = trunc_correction(p->c_in);
-  const int n_tiles = g.batch * g.tiles_y * g.tiles_x * g.groups;
-  const int grid = n_tiles < kNumSMs ? n_tiles : kNumSMs;
-  D3B_CUDA(launch_maybe_pdl(bev_conv16_kernel<KS, STRIDE, COUT>, dim3(grid), dim3(kBvThreads), Cfg::kSmemBytes, stream, tm_hi,
-                            tm_lo, g, (const __half*)p->weight_packed, e, (__half*)p->out_hi, (__half*)p->out_lo, p->out_f32,
-                            (int*)p->overflow));
-  D3B_LAUNCH_CHECK();
-  return D3B_OK;
-}
-
-// channel-stationary variant: 3x3, stride 1, one or more output blocks of exactly 128 channels, no sub-pixel groups
-static int launch_bev_cs(const d3b_bev16_params* p, const BvGeom& g, cudaStream_t stream) {
-  static SmemOptIn optin;
-  D3B_CUDA(ensure_dynamic_smem(bev_conv16_cs_kernel, kBwSmemBytes, optin));
-  CUtensorMap tm_hi, tm_lo;
-  int st = make_map(&tm_hi, p->in_hi, p->batch, p->h_in, p->w_in, p->c_in, kBvTileX, kBwPatchRows, 1);
-  if (st != D3B_OK) return st;
-  st = make_map(&tm_lo, p->in_lo, p->batch, p->h_in, p->w_in, p->c_in, kBvTileX, kBwPatchRows, 1);
-  if (st != D3B_OK) return st;
-  BvEpi e;
-  e.bias = p->bias; e.scale = p->scale; e.shift = p->shift; e.acc_scale = p->acc_scale; e.relu = p->relu;
-  e.corr = trunc_correction(p->c_in);
-  const int n_tiles = g.batch * g.tiles_y * g.tiles_x * g.groups;
-  const int grid = n_tiles < kNumSMs ? n_tiles : kNumSMs;
-  D3B_CUDA(launch_maybe_pdl(bev_conv16_cs_kernel, dim3(grid), dim3(kBwThreads), kBwSmemBytes, stream, tm_hi, tm_lo, g,
-                            (const __half*)p->weight_packed, e, (__half*)p->out_hi, (__half*)p->out_lo, p->out_f32,
-                            (int*)p->overflow));
+  D3B_CUDA(launch_maybe_pdl(bev_conv16_kernel<KS, STRIDE, COUT>, dim3(bev_grid(g)), dim3(kBvThreads), Cfg::kSmemBytes,
+                            stream, tm_hi, tm_lo, g, (const __half*)p->weight_packed, e, (__half*)p->out_hi,
+                            (__half*)p->out_lo, p->out_f32, (int*)p->overflow));
   D3B_LAUNCH_CHECK();
   return D3B_OK;
 }
@@ -770,18 +545,12 @@ static int launch_bev_pl(const d3b_bev16_params* p, BvGeom g, cudaStream_t strea
   static SmemOptIn optin;
   D3B_CUDA(ensure_dynamic_smem(bev_conv16_pl_kernel, kPlSmemBytes, optin));
   CUtensorMap tm_hi, tm_lo;
-  int st = make_map(&tm_hi, p->in_hi, p->batch, p->h_in, p->w_in, p->c_in, kBvHalfX, kBvTileY + 2, 1);
+  Epi16 e;
+  const int st = bev_args(p, kBvHalfX, kBvTileY + 2, 1, &tm_hi, &tm_lo, &e);
   if (st != D3B_OK) return st;
-  st = make_map(&tm_lo, p->in_lo, p->batch, p->h_in, p->w_in, p->c_in, kBvHalfX, kBvTileY + 2, 1);
-  if (st != D3B_OK) return st;
-  BvEpi e;
-  e.bias = p->bias; e.scale = p->scale; e.shift = p->shift; e.acc_scale = p->acc_scale; e.relu = p->relu;
-  e.corr = trunc_correction(p->c_in);
   g.tiles_x = div_up(g.w_out, kBvHalfX);     // tiles of 16 rows x 8 columns
-  const int n_tiles = g.batch * g.tiles_y * g.tiles_x * g.groups;
-  const int grid = n_tiles < kNumSMs ? n_tiles : kNumSMs;
-  D3B_CUDA(launch_maybe_pdl(bev_conv16_pl_kernel, dim3(grid), dim3(kBvThreads), kPlSmemBytes, stream, tm_hi, tm_lo, g,
-                            (const __half*)p->weight_packed, e, (__half*)p->out_hi, (__half*)p->out_lo, p->out_f32,
+  D3B_CUDA(launch_maybe_pdl(bev_conv16_pl_kernel, dim3(bev_grid(g)), dim3(kBvThreads), kPlSmemBytes, stream, tm_hi, tm_lo,
+                            g, (const __half*)p->weight_packed, e, (__half*)p->out_hi, (__half*)p->out_lo, p->out_f32,
                             (int*)p->overflow));
   D3B_LAUNCH_CHECK();
   return D3B_OK;
@@ -827,15 +596,11 @@ extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
   g.groups = p->groups; g.cgroups = p->cgroups; g.up = p->up;
   g.out_h = g.h_out * p->up; g.out_w = g.w_out * p->up;
   g.out_channels = p->out_channels; g.out_c0 = p->out_c0;
-  static std::atomic<int> launch_seq{0};
-  g.seq = launch_seq.fetch_add(1, std::memory_order_relaxed);
   // Automatic (variant 2) = the pipelined kernel for the 3x3 stride-1 layers with 128-channel output blocks, the
-  // pixel-stationary kernel for every other shape.  Variant 0 (pixel-stationary everywhere) is the reference the other
-  // two reproduce bit for bit; variant 1 selects the channel-stationary kernel for the 3x3 stride-1 layers.
-  const int variant = bev_variant();
-  const bool s1_blocks = p->ksize == 3 && p->stride == 1 && p->c_out == kBwCout && p->c_in % kBvKc == 0 && p->up == 1;
-  if (variant == 1 && s1_blocks && p->out_channels % 4 == 0) return launch_bev_cs(p, g, stream);
-  if (variant == 2 && s1_blocks) return launch_bev_pl(p, g, stream);
+  // pixel-stationary kernel for every other shape.  Variant 0 (pixel-stationary everywhere) is the reference the
+  // pipelined kernel reproduces bit for bit.
+  const bool s1_blocks = p->ksize == 3 && p->stride == 1 && p->c_out == kPlCout && p->c_in % kBvKc == 0 && p->up == 1;
+  if (bev_variant() == 2 && s1_blocks) return launch_bev_pl(p, g, stream);
 #define D3B_BEV_CASE(KS, ST)                                                   \
   if (p->ksize == KS && p->stride == ST) {                                     \
     switch (p->c_out) {                                                        \

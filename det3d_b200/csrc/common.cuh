@@ -76,9 +76,9 @@ int nms_batched(int fmt_kernel, const float* boxes, int n_cap, const int* n_dev,
 // blocks until kernel N has completed and its writes are visible.  Inside a captured CUDA graph the edge becomes a
 // programmatic dependency.  d3b_set_pdl(0) turns it off (plain stream order).
 bool pdl_enabled();
-// bevconv16_sm90.cu: 0 = pixel-stationary tiles (two 128-pixel halves) everywhere, 1 = channel-stationary kernel for the
-// 3x3 stride-1 128-channel-block layers, 2 = automatic = the pipelined kernel (16 x 8 pixel tiles, two partials in
-// flight) for those layers and pixel-stationary for the rest, the fastest choice on the H100 (d3b_set_bev_variant)
+// bevconv16_sm90.cu: 0 = pixel-stationary tiles (two 128-pixel halves) everywhere, 2 = automatic = the pipelined kernel
+// (16 x 8 pixel tiles, two partials in flight) for the 3x3 stride-1 128-channel-block layers and pixel-stationary for
+// the rest, the fastest choice on the H100 (d3b_set_bev_variant)
 int bev_variant();
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_maybe_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,

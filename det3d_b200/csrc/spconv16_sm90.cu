@@ -35,7 +35,7 @@
 // arrive by cp.async.bulk; the kernel is launched with programmatic stream serialisation (prologue overlaps the
 // previous layer's tail).
 // Algorithmic bytes per layer (SURVEY 8d): N_in*C_in*4 + N_out*C_out*4 + P*8 + K*C_in*C_out*4.
-#include "gmma.cuh"
+#include "epilogue16.cuh"
 
 namespace d3b {
 
@@ -64,24 +64,9 @@ struct OsCfg {
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/ + 32 * kOsTileM * 4;
 };
 
-__device__ __forceinline__ uint32_t pack_half2(__half a, __half b) {
-  return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
-}
-
-// Fused epilogue on 16 consecutive output channels of one row; returns true if a value left the f16 range.
-struct OsEpi {
-  const float* bias;
-  const float* scale;
-  const float* shift;
-  const __half* res_hi;
-  const __half* res_lo;
-  float acc_scale;
-  float corr;                     // mean truncation of the layer's partials (gmma.cuh), applied to the sums
-  int relu;
-  int seq;                        // launch counter of this translation unit (development traces only)
-};
-
-__device__ __forceinline__ bool epilogue16(float (&v)[16], const OsEpi& e, size_t row_off, int col, __half* out_hi,
+// Fused epilogue on 16 consecutive output channels of one row (the FFMA first layer: its sums are not truncated, so no
+// correction); returns true if a value left the f16 range.
+__device__ __forceinline__ bool epilogue16(float (&v)[16], const Epi16& e, size_t row_off, int col, __half* out_hi,
                                            __half* out_lo, float* out_f32) {
 #pragma unroll
   for (int q = 0; q < 16; ++q) v[q] *= e.acc_scale;
@@ -124,14 +109,7 @@ __device__ __forceinline__ bool epilogue16(float (&v)[16], const OsEpi& e, size_
   if (out_hi) {
     uint32_t hi[8], lo[8];
 #pragma unroll
-    for (int q = 0; q < 16; q += 2) {
-      __half h0, l0, h1, l1;
-      split_f16(v[q], h0, l0);
-      split_f16(v[q + 1], h1, l1);
-      hi[q >> 1] = pack_half2(h0, h1);
-      lo[q >> 1] = pack_half2(l0, l1);
-      ovf |= !(fabsf(v[q]) < 65504.f) | !(fabsf(v[q + 1]) < 65504.f);
-    }
+    for (int q = 0; q < 16; q += 2) ovf |= split_pack2(v[q], v[q + 1], hi[q >> 1], lo[q >> 1]);
     uint4* ph = reinterpret_cast<uint4*>(out_hi + row_off + col);
     uint4* pl = reinterpret_cast<uint4*>(out_lo + row_off + col);
     ph[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
@@ -147,8 +125,8 @@ __device__ __forceinline__ bool epilogue16(float (&v)[16], const OsEpi& e, size_
   return ovf;
 }
 
-// The same epilogue on the two consecutive output channels a wgmma accumulator fragment holds.
-__device__ __forceinline__ bool epilogue2(float v0, float v1, const OsEpi& e, size_t row_off, int col, __half* out_hi,
+// The same epilogue on the two consecutive output channels a wgmma accumulator fragment holds, with the correction.
+__device__ __forceinline__ bool epilogue2(float v0, float v1, const Epi16& e, size_t row_off, int col, __half* out_hi,
                                           __half* out_lo, float* out_f32) {
   v0 *= e.acc_scale;
   v1 *= e.acc_scale;
@@ -172,12 +150,10 @@ __device__ __forceinline__ bool epilogue2(float v0, float v1, const OsEpi& e, si
   if (e.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
   bool ovf = false;
   if (out_hi) {
-    __half h0, l0, h1, l1;
-    split_f16(v0, h0, l0);
-    split_f16(v1, h1, l1);
-    *reinterpret_cast<uint32_t*>(out_hi + row_off + col) = pack_half2(h0, h1);
-    *reinterpret_cast<uint32_t*>(out_lo + row_off + col) = pack_half2(l0, l1);
-    ovf = !(fabsf(v0) < 65504.f) | !(fabsf(v1) < 65504.f);
+    uint32_t hi, lo;
+    ovf = split_pack2(v0, v1, hi, lo);
+    *reinterpret_cast<uint32_t*>(out_hi + row_off + col) = hi;
+    *reinterpret_cast<uint32_t*>(out_lo + row_off + col) = lo;
   }
   if (out_f32) *reinterpret_cast<float2*>(out_f32 + row_off + col) = make_float2(v0, v1);
   return ovf;
@@ -203,7 +179,7 @@ template <int COUT>
 __global__ void __launch_bounds__(OsCfg<COUT>::kThreads, 1)
 spconv_os16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ in_lo, const int* __restrict__ nbr,
                    const unsigned int* __restrict__ tile_mask, const int* __restrict__ n_out_p, int out_cap, int c_in,
-                   int n_kb, int pack, int k_vol, const __half* __restrict__ packed, OsEpi epi, __half* __restrict__ out_hi,
+                   int n_kb, int pack, int k_vol, const __half* __restrict__ packed, Epi16 epi, __half* __restrict__ out_hi,
                    __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
   using Cfg = OsCfg<COUT>;
   extern __shared__ uint8_t smem_raw[];
@@ -402,7 +378,7 @@ spconv_os16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ 
 template <int COUT>
 __global__ void __launch_bounds__(256)
 spconv_first16_kernel(const float* __restrict__ feat_in, const int* __restrict__ nbr, const int* __restrict__ n_out_p,
-                      int out_cap, int c_in, int k_vol, const float* __restrict__ weight, OsEpi epi,
+                      int out_cap, int c_in, int k_vol, const float* __restrict__ weight, Epi16 epi,
                       __half* __restrict__ out_hi, __half* __restrict__ out_lo, float* __restrict__ out_f32,
                       int* __restrict__ overflow) {
   extern __shared__ float w_s[];                 // [k_vol][c_in][COUT]
@@ -482,12 +458,7 @@ split16_kernel(const float* __restrict__ x, long long n, __half* __restrict__ hi
                int* __restrict__ overflow) {
   bool ovf = false;
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
-    const float v = x[e];
-    __half h, l;
-    split_f16(v, h, l);
-    hi[e] = h;
-    lo[e] = l;
-    ovf |= !(fabsf(v) < 65504.f);
+    ovf |= store16(x[e], hi + e, lo + e);
   }
   if (ovf && overflow) atomicOr(overflow, 1);
 }
@@ -519,12 +490,7 @@ sparse_to_bev16_kernel(const __half* __restrict__ in_hi, const __half* __restric
       continue;
     const size_t dst = (((size_t)q.x * H + q.z) * W + q.w) * ((size_t)C * D) + (size_t)c * D + q.y;
     if (in_f32) {
-      const float v = in_f32[e];
-      __half h, l;
-      split_f16(v, h, l);
-      out_hi[dst] = h;
-      out_lo[dst] = l;
-      if (!(fabsf(v) < 65504.f) && overflow) {
+      if (store16(in_f32[e], out_hi + dst, out_lo + dst) && overflow) {
         if ((__activemask() & ((1u << (threadIdx.x & 31)) - 1u)) == 0u) atomicOr(overflow, 1);
       }
     } else {
@@ -540,8 +506,8 @@ static bool os16_shape_ok(int c_in, int c_out) {
   return cin_ok && cout_ok;
 }
 
-static OsEpi epi_of(const d3b_conv16_params* p) {
-  OsEpi e;
+static Epi16 epi_of(const d3b_conv16_params* p) {
+  Epi16 e;
   e.bias = p->bias; e.scale = p->scale; e.shift = p->shift;
   e.res_hi = (const __half*)p->residual_hi; e.res_lo = (const __half*)p->residual_lo;
   e.acc_scale = p->acc_scale; e.relu = p->relu;
@@ -561,7 +527,7 @@ static int launch_os16(const d3b_conv16_params* p, const int32_t* nbr, const uin
   const int grid = n_tiles < kNumSMs ? (n_tiles > 0 ? n_tiles : 1) : kNumSMs;
   const int pack = os16_pack(p->c_in, p->k_vol);
   const int n_kb = pack > 1 ? 1 : (p->c_in + kOsKc - 1) / kOsKc;
-  OsEpi epi = epi_of(p);
+  Epi16 epi = epi_of(p);
   epi.corr = trunc_correction(p->c_in * pack);
   D3B_CUDA(launch_maybe_pdl(spconv_os16_kernel<COUT>, dim3(grid), dim3(Cfg::kThreads), Cfg::kSmemBytes, stream,
                             (const __half*)p->in_hi, (const __half*)p->in_lo, (const int*)nbr, (const unsigned int*)tile_mask,

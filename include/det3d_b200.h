@@ -40,11 +40,10 @@ unsigned long long d3b_launch_count(void);
  * launch latency and prologue overlap the previous kernel's tail; results are unaffected. 0 = plain stream order. */
 void d3b_set_pdl(int on);
 /* Schedule of d3b_bev_conv16 for 3x3 stride-1 layers whose output blocks are 128 channels wide (the RPN blocks of
- * necks/rpn.py:124-142): 0 = pixel-stationary (two 128-pixel halves per 16 x 16 pixel tile), 1 = channel-stationary
- * (C_out as the wgmma M dimension, the 256 tile pixels as N), 2 = automatic (default: the pipelined kernel -- 16 x 8
- * pixel tiles, one m64n128 chain per kernel offset, two partials in flight -- for such layers whose C_in is a multiple
- * of 64, the pixel-stationary kernel otherwise; measured the fastest on the H100).  Same products in the same order:
- * the results are bit-identical. */
+ * necks/rpn.py:124-142): 0 = pixel-stationary (two 128-pixel halves per 16 x 16 pixel tile), 2 = automatic (default:
+ * the pipelined kernel -- 16 x 8 pixel tiles, one m64n128 chain per kernel offset, two partials in flight -- for such
+ * layers whose C_in is a multiple of 64, the pixel-stationary kernel otherwise; measured the fastest on the H100).  Any
+ * other value selects 2.  Same products in the same order: the results are bit-identical. */
 void d3b_set_bev_variant(int variant);
 int d3b_get_bev_variant(void);
 

@@ -165,46 +165,3 @@ def test_bev_conv16_transpose_into_concat_slice(up, c_in, c_out, h, w):
     got = out.to_f32()
     assert float(got[..., :64].abs().max()) == 0.0                       # the neighbouring slice is untouched
     assert float((got[..., 64:] - _nhwc(want)).abs().max()) <= TOL
-
-
-@pytest.mark.parametrize("b,h,w,c_in,c_out", [
-    (1, 200, 176, 128, 128),      # SECOND RPN layer: 143 tiles, one per CTA
-    (2, 37, 29, 64, 128),         # ragged grid, two samples, one 64-channel slice
-    (1, 40, 40, 256, 256),        # two output blocks of 128, four input slices
-    (5, 64, 48, 128, 128),        # more tiles than SMs: CTAs walk several tiles (buffer / stage parities carry over)
-])
-def test_bev_conv16_channel_stationary_variant(b, h, w, c_in, c_out):
-    """d3b_set_bev_variant(1): the transposed schedule (C_out as the wgmma M dimension, the tile's pixels as N)
-    against float64 conv2d and against the pixel-stationary schedule (same products, same order, same chains)."""
-    from det3d_b200 import _lib
-    from det3d_b200.ops.spconv import conv16
-    torch.manual_seed(h * 11 + c_out)
-    x = torch.randn((b, c_in, h, w), device="cuda")
-    wt = torch.randn((c_out, c_in, 3, 3), device="cuda") * (1.0 / np.sqrt(9 * c_in * 0.3))
-    bias = torch.randn(c_out, device="cuda") * 0.1
-    scale = torch.rand(c_out, device="cuda") + 0.5
-    shift = torch.randn(c_out, device="cuda") * 0.1
-    want = F.conv2d(x.double(), wt.double(), bias=bias.double(), padding=1)
-    want = torch.relu(want * scale.double().view(1, -1, 1, 1) + shift.double().view(1, -1, 1, 1)).float()
-    layer = conv16.BevConv16(wt.permute(2, 3, 1, 0).reshape(9, c_in, c_out), 3, stride=1, pad=1, bias=bias, scale=scale,
-                             shift=shift, relu=True, device="cuda")
-    xin = conv16.Planes.from_f32(_nhwc(x))
-    total = c_out + 32                      # written into a channel slice of a wider buffer
-    outs = {}
-    prev = _lib.lib().d3b_get_bev_variant()
-    try:
-        for variant in (0, 1):
-            _lib.lib().d3b_set_bev_variant(variant)
-            out = conv16.Planes((b, h, w, total), "cuda", zero=True)
-            out_f32 = torch.zeros((b, h, w, total), device="cuda")
-            ovf = torch.zeros(1, dtype=torch.int32, device="cuda")
-            layer(xin, out=out, out_f32=out_f32, out_c0=32, overflow=ovf)
-            assert int(ovf.item()) == 0
-            outs[variant] = (out, out_f32)
-    finally:
-        _lib.lib().d3b_set_bev_variant(prev)
-    out, out_f32 = outs[1]
-    assert float(out_f32[..., :32].abs().max()) == 0.0 and float(out.to_f32()[..., :32].abs().max()) == 0.0
-    assert float((out_f32[..., 32:] - _nhwc(want)).abs().max()) <= TOL
-    assert float((out.to_f32()[..., 32:] - _nhwc(want)).abs().max()) <= TOL
-    assert torch.equal(out_f32, outs[0][1]) and torch.equal(out.buf, outs[0][0].buf)

@@ -246,7 +246,7 @@ def operands(a_shape, w_shape, regime, gen, a_scale=1.0, w_max=None):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# dense (pixel- and channel-stationary FP16x3)
+# dense (pixel-stationary and pipelined FP16x3)
 # ---------------------------------------------------------------------------------------------------------------------
 
 def dense_ref(x, planes, wt, w_exp, ks, stride, pad, up):
@@ -457,9 +457,9 @@ def test_sparse_fp16x3_epilogue_and_planes():
 
 
 @pytest.mark.parametrize("c_in,b,c_out", [(64, 1, 128), (192, 3, 128), (256, 8, 256), (128, 3, 256)])
-def test_channel_stationary_bit_identical(c_in, b, c_out):
-    """Channel-stationary schedule (selected for 3x3 / stride 1 / 128-channel blocks / C_in % 64 == 0) gives the bits
-    of the pixel-stationary one, on more C_in multiples of 64 and batch sizes, with a ragged grid."""
+def test_pipelined_bit_identical(c_in, b, c_out):
+    """The pipelined schedule (the automatic choice for 3x3 / stride 1 / 128-channel blocks / C_in % 64 == 0) gives the
+    bits of the pixel-stationary one, on more C_in multiples of 64 and batch sizes, with a ragged grid."""
     from det3d_b200 import _lib
     from det3d_b200.ops.spconv import conv16
     gen = torch.Generator(device="cuda").manual_seed(c_in + b)
@@ -470,7 +470,7 @@ def test_channel_stationary_bit_identical(c_in, b, c_out):
     outs = []
     prev = _lib.lib().d3b_get_bev_variant()
     try:
-        for variant in (0, 1):
+        for variant in (0, 2):
             _lib.lib().d3b_set_bev_variant(variant)
             out = conv16.Planes((b, 21, 35, c_out), "cuda", zero=True)
             out32 = torch.zeros((b, 21, 35, c_out), device="cuda")
@@ -531,7 +531,7 @@ def test_overflow_flag_boundary():
             conv16.sparse_conv16(xin, rb, cw, None, out_f32=torch.empty((300, 128), device="cuda"), overflow=flag)
             assert int(flag.item()) == 0, "sparse out_f32-only launch raised the flag (v = %r)" % v
             layer = dense_layer(torch.zeros((1, 9, 64, 128), device="cuda"), 3, 1, 1, 1, bias=bias)
-            for variant in (0, 1):
+            for variant in (0, 2):
                 _lib.lib().d3b_set_bev_variant(variant)
                 flag.zero_()
                 layer(grid, out=conv16.Planes((1, 9, 11, 128), "cuda"), overflow=flag)
@@ -578,7 +578,7 @@ def test_sparse_rows_independent_of_row_order(c_in, c_out):
     assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1])
 
 
-@pytest.mark.parametrize("ks,stride,up,variant", [(3, 1, 1, 0), (3, 1, 1, 1), (3, 2, 1, 0), (1, 1, 2, 0)])
+@pytest.mark.parametrize("ks,stride,up,variant", [(3, 1, 1, 0), (3, 1, 1, 2), (3, 2, 1, 0), (1, 1, 2, 0)])
 def test_dense_sample_independent_of_batch(ks, stride, up, variant):
     """Sample s alone (B = 1) and at position 1 of a B = 3 batch: the same bits (H = 37, W = 29 are not multiples of 16,
     so tiles reach past the sample border, where the TMA fill must be zeros, not the next sample)."""
@@ -623,7 +623,7 @@ def bias_case(kernel, regime, seed=0):
         return got, ref
     prev = _lib.lib().d3b_get_bev_variant()
     try:
-        _lib.lib().d3b_set_bev_variant(1 if kernel == "dense_cs" else 0)
+        _lib.lib().d3b_set_bev_variant(2 if kernel == "dense_pl" else 0)
         got, ref, *_ = run_dense(1, 96, 88, 128, 128, 3, 1, 1, 1, 23 + seed, regime=regime)
     finally:
         _lib.lib().d3b_set_bev_variant(prev)
@@ -634,7 +634,7 @@ BIAS_B = 3 * EPS          # regime B (what the network feeds): a quarter of the 
 BIAS_ALL = 12 * EPS       # every regime: never worse than no correction at all
 
 
-@pytest.mark.parametrize("kernel", ["sparse", "dense_ps", "dense_cs"])
+@pytest.mark.parametrize("kernel", ["sparse", "dense_ps", "dense_pl"])
 @pytest.mark.parametrize("regime", ["A", "B", "C"])
 def test_truncation_correction_bias(kernel, regime):
     """Residual slope of the kernel against yh over a large launch.  The FP16x3 kernels are deterministic, so on seeded

@@ -3,8 +3,8 @@ triggers in the detectors.
 
 Kernel level.  Every plane writer -- d3b_split16, the pillar scatter d3b_sparse_to_bev16 (fp32 rows and plane rows),
 the fp32-input first sparse layer, the tensor-core sparse kernel at every C_out, and the dense kernel in each shape it
-builds (3x3 stride 1 / 2, 1x1, ConvTranspose, k = s deblocks, the channel-stationary schedule, a two-group launch into a
-channel slice) -- is driven across the boundary of the f16 range, with and without ReLU.  The value is placed on one
+builds (3x3 stride 1 / 2, 1x1, ConvTranspose, k = s deblocks, a two-group launch into a channel slice; the pipelined
+schedule in test_bev_conv16_pipelined_gpu) -- is driven across the boundary of the f16 range, with and without ReLU.  The value is placed on one
 output channel whose weights are zero, through the bias (scaled by an exact 1/2 in the folded BatchNorm, with a residual
 of 1 on the sparse kernel), so it reaches the range check exactly; the other channels carry ordinary O(1) results.  At
 every value the flag must be raised exactly when the value written is not below 65504 in magnitude or is NaN; hi / lo
@@ -231,9 +231,7 @@ DENSE = [
     ("k = s = 2", 2, 2, 0, 1, 64, 128, 0, 0, 0, 3),
     ("k = s = 3", 3, 3, 0, 1, 64, 64, 0, 0, 0, 40),
     ("k = s = 4", 4, 4, 0, 1, 128, 32, 0, 0, 0, 17),
-    ("channel-stationary", 3, 1, 1, 1, 128, 128, 1, 0, 0, 90),
     ("cgroups 2 into a slice", 3, 1, 1, 1, 64, 256, 0, 64, 64, 128 + 9),
-    ("cgroups 2 into a slice, channel-stationary", 3, 1, 1, 1, 64, 256, 1, 64, 64, 128 + 9),
 ]
 
 

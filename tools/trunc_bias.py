@@ -7,7 +7,7 @@ reference, and the residual slope
     beta = sum (got - ref) ref / sum ref^2
 
 is printed with its standard error, in units of eps = 2^-26 (kTruncLossPerMma in csrc/gmma.cuh).  The FP16x3 kernels
-(sparse output-stationary, dense pixel- and channel-stationary) are measured against the split-exact result yh of the
+(sparse output-stationary, dense pixel-stationary and pipelined) are measured against the split-exact result yh of the
 operands they see (tests/test_conv_error_model_gpu.py): each full slot chains n = 12 truncating MMAs and the epilogue
 adds 12 eps (kTruncLossPerMma per MMA) to the sums, so the true mean loss per MMA is about (12 eps - beta) / 12.  The tf32x3
 fallback kernels (simt, tc, pairs; tc over a dense rulebook) are measured against the exact y at features ~3e5.
@@ -76,7 +76,7 @@ def main():
     print("gpu: %s" % info)
     rows = []
     eps = em.EPS
-    for kernel in ("sparse", "dense_ps", "dense_cs"):
+    for kernel in ("sparse", "dense_ps", "dense_pl"):
         for regime in ("A", "B", "C"):
             got, ref = em.bias_case(kernel, regime)
             beta, se = em.residual_slope(got, ref.yh)
