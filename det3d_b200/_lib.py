@@ -14,7 +14,6 @@ LIB_PATH = os.environ.get("D3B_LIB") or os.path.join(_HERE, "lib", "libdet3d_b20
 D3B_OK = 0
 ALGO_SIMT = 0
 ALGO_TC = 1
-ALGO_TC_PAIRS = 2
 AA_IOU3D, AA_PIXEL = 0, 1
 BOX_XYXYR = 0
 BOX_XYWLR = 1
@@ -62,14 +61,6 @@ class ConvParams(C.Structure):
         ("residual", C.c_void_p),
         ("relu", C.c_int32),
         ("algo", C.c_int32),
-        ("pair_in", C.c_void_p),
-        ("pair_out", C.c_void_p),
-        ("pair_count", C.c_void_p),
-        ("in_bias", C.c_void_p),
-        ("in_scale", C.c_void_p),
-        ("in_shift", C.c_void_p),
-        ("in_relu", C.c_int32),
-        ("out_zeroed", C.c_int32),
     ]
 
 
@@ -134,14 +125,11 @@ SIGNATURES = {
     "d3b_ingest_sweeps_gather": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _sz, _vp]),
     "d3b_rulebook_workspace_bytes": (_sz, [_i64]),
     "d3b_index_build_hash": (C.c_int, [_vp, _vp, _i32, C.POINTER(SiteIndex), _vp]),
-    "d3b_rulebook_subm": (C.c_int, [_vp, _vp, _i32, C.POINTER(SiteIndex), _I3, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "d3b_rulebook_conv": (C.c_int, [_vp, _vp, _i32, C.POINTER(SiteIndex), _I3, _I3, _I3, C.POINTER(SiteIndex), _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "d3b_rulebook_subm": (C.c_int, [_vp, _vp, _i32, C.POINTER(SiteIndex), _I3, _vp, _vp, _vp]),
+    "d3b_rulebook_conv": (C.c_int, [_vp, _vp, _i32, C.POINTER(SiteIndex), _I3, _I3, _I3, C.POINTER(SiteIndex), _vp, _vp, _i32, _vp, _vp, _vp, _sz, _vp]),
     "d3b_conv_packed_weight_floats": (_sz, [_i32, _i32, _i32]),
     "d3b_conv_pack_weight": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp]),
     "d3b_sparse_conv": (C.c_int, [_vp, _vp, _vp, _vp, _i32, C.POINTER(ConvParams), _vp, _vp]),
-    "d3b_rulebook_pairs": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp]),
-    "d3b_zero_rows": (C.c_int, [_vp, _vp, _i32, _vp, _i32, _vp]),
-    "d3b_feature_epilogue": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _vp]),
     "d3b_sparse_to_dense": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _I3, _i32, _vp, _vp]),
     "d3b_pillar_features": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, C.c_float, C.c_float, C.c_float, C.c_float, _vp, _vp]),
     "d3b_voxelize_point_lists": (_vp, [C.POINTER(VoxelCfg), _i32, _i32, _vp]),

@@ -99,7 +99,8 @@ class InferencePipeline:
 
     def check_overflow(self, flag_value):
         """Host side of the guard: on a raised flag switch the model to the tf32x3 kernels (permanently: the weights /
-        inputs that overflowed once will again) and tell the caller to re-run.  Returns True if a re-run is needed."""
+        inputs that overflowed once will again) and tell the caller to re-run.  Returns True if a re-run is needed.
+        The tf32x3 kernels are output-stationary like the FP16x3 ones, so re-run results are reproducible bit for bit."""
         if not flag_value:
             return False
         warnings.warn("det3d_b200: a feature left the f16 range (|x| >= 65504); re-running on the tf32x3 kernels")

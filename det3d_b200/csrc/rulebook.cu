@@ -104,8 +104,7 @@ rb_hash_insert(const int* __restrict__ coors, const int* __restrict__ n_rows, in
 __global__ void __launch_bounds__(256)
 rb_neighbours(const int* __restrict__ out_coors, const int* __restrict__ n_out, int out_cap,
               SiteIndexDev in_index, KernelGeom g, int* __restrict__ nbr,
-              unsigned int* __restrict__ tile_mask, int* __restrict__ pair_in, int* __restrict__ pair_out,
-              int* __restrict__ pair_count) {
+              unsigned int* __restrict__ tile_mask) {
   const int n = min(*n_out, out_cap);
   const long long total = (long long)n * g.kvol;
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total;
@@ -126,21 +125,6 @@ rb_neighbours(const int* __restrict__ out_coors, const int* __restrict__ n_out, 
       const int tag = (o >> 7) * 32 + k;
       const unsigned int peers = __match_any_sync(__activemask(), tag);
       if ((int)(__ffs(peers) - 1) == (int)(threadIdx.x & 31)) atomicOr(&tile_mask[o >> 7], 1u << k);
-    }
-    if (pair_count != nullptr) {
-      // classic rulebook form for the pair-based kernel: the warp's valid entries of one offset take
-      // consecutive slots through one aggregated atomicAdd (pair order inside an offset is arbitrary)
-      const int lane = threadIdx.x & 31;
-      const unsigned int grp = __match_any_sync(__activemask(), r >= 0 ? k : -1);   // misses share one tag
-      if (r >= 0) {
-        const int leader = __ffs(grp) - 1;
-        int base = 0;
-        if (lane == leader) base = atomicAdd(&pair_count[k], __popc(grp));
-        base = __shfl_sync(grp, base, leader);
-        const int pos = base + __popc(grp & ((1u << lane) - 1u));
-        pair_in[(size_t)k * out_cap + pos] = r;
-        pair_out[(size_t)k * out_cap + pos] = o;
-      }
     }
   }
 }
@@ -299,37 +283,6 @@ rb_emit_coors(const unsigned int* __restrict__ bitmap, const int* __restrict__ w
   }
 }
 
-// ---- pair lists (classic rulebook form) ---------------------------------------------------
-// One thread per (k, o); a warp's valid entries of the same k take consecutive slots through one
-// warp-aggregated atomicAdd.  Pair order inside an offset is therefore arbitrary (as in spconv's GPU
-// rulebook); only the fp32 summation order of the atomics-based kernel depends on it.
-__global__ void __launch_bounds__(256)
-rb_compact_pairs(const int* __restrict__ nbr, const int* __restrict__ n_out, int out_cap, int k_vol,
-                 int* __restrict__ pair_in, int* __restrict__ pair_out, int* __restrict__ pair_count) {
-  const int n = min(*n_out, out_cap);
-  const long long total = (long long)n * k_vol;
-  for (long long e0 = (long long)blockIdx.x * blockDim.x; e0 < total; e0 += (long long)gridDim.x * blockDim.x) {
-    const long long e = e0 + threadIdx.x;
-    int k = -1, o = 0, src = -1;
-    if (e < total) {
-      k = (int)(e / n);
-      o = (int)(e - (long long)k * n);
-      src = nbr[(size_t)k * out_cap + o];
-    }
-    const bool valid = src >= 0;
-    const unsigned int peers = __match_any_sync(0xffffffffu, valid ? k : -1);
-    if (valid) {
-      const int leader = __ffs(peers) - 1;
-      int base = 0;
-      if ((int)(threadIdx.x & 31) == leader) base = atomicAdd(&pair_count[k], __popc(peers));
-      base = __shfl_sync(peers, base, leader);
-      const int pos = base + __popc(peers & ((1u << (threadIdx.x & 31)) - 1u));
-      pair_in[(size_t)k * out_cap + pos] = src;
-      pair_out[(size_t)k * out_cap + pos] = o;
-    }
-  }
-}
-
 static int check_geom(const int32_t ksize[3], KernelGeom* g) {
   g->kvol = ksize[0] * ksize[1] * ksize[2];
   for (int j = 0; j < 3; ++j) g->k[j] = ksize[j];
@@ -363,17 +316,9 @@ extern "C" int d3b_index_build_hash(const int32_t* coors, const int32_t* n_rows,
   return D3B_OK;
 }
 
-static int clear_pairs(int32_t* pair_in, int32_t* pair_out, int32_t* pair_count, int k_vol, cudaStream_t stream) {
-  if (pair_count == nullptr) return D3B_OK;
-  D3B_REQUIRE(pair_in && pair_out, "rulebook: pair_in / pair_out must accompany pair_count");
-  D3B_CUDA(cudaMemsetAsync(pair_count, 0, (size_t)k_vol * 4, stream));
-  return D3B_OK;
-}
-
 extern "C" int d3b_rulebook_subm(const int32_t* coors, const int32_t* n_rows, int32_t row_cap,
                                  const d3b_site_index* index, const int32_t ksize[3], int32_t* nbr,
-                                 uint32_t* tile_mask, int32_t* pair_in, int32_t* pair_out,
-                                 int32_t* pair_count, void* stream_) {
+                                 uint32_t* tile_mask, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   D3B_REQUIRE(coors && n_rows && index && ksize && nbr && tile_mask, "d3b_rulebook_subm: null argument");
   KernelGeom g;
@@ -384,22 +329,8 @@ extern "C" int d3b_rulebook_subm(const int32_t* coors, const int32_t* n_rows, in
     g.p[j] = ksize[j] / 2;
   }
   D3B_CUDA(cudaMemsetAsync(tile_mask, 0, (size_t)div_up(row_cap, 128) * 4, stream));
-  { const int st = clear_pairs(pair_in, pair_out, pair_count, g.kvol, stream); if (st != D3B_OK) return st; }
   rb_neighbours<<<grid_for((long long)row_cap * g.kvol, 256), 256, 0, stream>>>(
-      coors, n_rows, row_cap, to_dev(index, row_cap), g, nbr, tile_mask, pair_in, pair_out, pair_count);
-  D3B_LAUNCH_CHECK();
-  return D3B_OK;
-}
-
-extern "C" int d3b_rulebook_pairs(const int32_t* nbr, const int32_t* n_out, int32_t out_cap, int32_t k_vol,
-                                  int32_t* pair_in, int32_t* pair_out, int32_t* pair_count, void* stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
-  D3B_REQUIRE(nbr && n_out && pair_in && pair_out && pair_count, "d3b_rulebook_pairs: null argument");
-  D3B_REQUIRE(k_vol >= 1 && k_vol <= 32 && out_cap >= 0, "d3b_rulebook_pairs: bad shape");
-  D3B_CUDA(cudaMemsetAsync(pair_count, 0, (size_t)k_vol * 4, stream));
-  if (out_cap == 0) return D3B_OK;
-  rb_compact_pairs<<<grid_for((long long)out_cap * k_vol, 256), 256, 0, stream>>>(nbr, n_out, out_cap, k_vol, pair_in,
-                                                                              pair_out, pair_count);
+      coors, n_rows, row_cap, to_dev(index, row_cap), g, nbr, tile_mask);
   D3B_LAUNCH_CHECK();
   return D3B_OK;
 }
@@ -408,8 +339,7 @@ extern "C" int d3b_rulebook_conv(const int32_t* in_coors, const int32_t* n_in, i
                                  const d3b_site_index* in_index, const int32_t ksize[3],
                                  const int32_t stride[3], const int32_t padding[3],
                                  d3b_site_index* out_index, int32_t* out_coors, int32_t* n_out,
-                                 int32_t out_cap, int32_t* nbr, uint32_t* tile_mask, int32_t* pair_in,
-                                 int32_t* pair_out, int32_t* pair_count, void* workspace,
+                                 int32_t out_cap, int32_t* nbr, uint32_t* tile_mask, void* workspace,
                                  size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   D3B_REQUIRE(in_coors && n_in && in_index && ksize && stride && padding && out_index &&
@@ -453,9 +383,8 @@ extern "C" int d3b_rulebook_conv(const int32_t* in_coors, const int32_t* n_in, i
   rb_emit_coors<<<grid_for(n_words, 256), 256, 0, stream>>>(out_index->bitmap, out_index->word_prefix, n_words, out,
                                                            out_cap, out_coors);
   D3B_LAUNCH_CHECK();
-  { const int st = clear_pairs(pair_in, pair_out, pair_count, g.kvol, stream); if (st != D3B_OK) return st; }
   rb_neighbours<<<grid_for((long long)out_cap * g.kvol, 256), 256, 0, stream>>>(
-      out_coors, n_out, out_cap, to_dev(in_index, in_cap), g, nbr, tile_mask, pair_in, pair_out, pair_count);
+      out_coors, n_out, out_cap, to_dev(in_index, in_cap), g, nbr, tile_mask);
   D3B_LAUNCH_CHECK();
   return D3B_OK;
 }

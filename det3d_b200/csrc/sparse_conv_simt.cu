@@ -21,9 +21,6 @@ int sparse_conv_tc(const float* feat_in, const int32_t* nbr, const uint32_t* til
                    const int32_t* n_out, int32_t out_cap, const d3b_conv_params* p,
                    float* feat_out, cudaStream_t stream);
 
-int sparse_conv_tc_pairs(const float* feat_in, const int32_t* n_out, int32_t out_cap, const d3b_conv_params* p,
-                         float* feat_out, cudaStream_t stream);
-
 constexpr int kTileM = 128;
 constexpr int kSimtThreads = 256;
 constexpr int kChunk = 16;  // input channels staged per step
@@ -225,10 +222,7 @@ extern "C" int d3b_sparse_conv(const float* feat_in, const int32_t* nbr, const u
                                float* feat_out, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   D3B_REQUIRE(feat_in && n_out && p && feat_out, "d3b_sparse_conv: null argument");
-  if (p->algo == D3B_ALGO_TC_PAIRS) {
-    if (out_cap == 0) return D3B_OK;
-    return sparse_conv_tc_pairs(feat_in, n_out, out_cap, p, feat_out, stream);
-  }
+  D3B_REQUIRE(p->algo == D3B_ALGO_SIMT || p->algo == D3B_ALGO_TC, "d3b_sparse_conv: unknown algo %d", p->algo);
   D3B_REQUIRE(nbr && tile_mask, "d3b_sparse_conv: null rulebook");
   D3B_REQUIRE(p->c_in >= 1 && p->c_out >= 1 && p->k_vol >= 1 && p->k_vol <= 32 && out_cap >= 0,
               "d3b_sparse_conv: bad shape (c_in %d c_out %d k_vol %d)", p->c_in, p->c_out, p->k_vol);

@@ -5,7 +5,7 @@
 // Reference: spconv v1.x indice_conv (per offset: gather -> fp32 torch.mm -> scatter-add) followed by
 // BatchNorm1d(eval) / ReLU / residual, call sites det3d/models/backbones/scn.py:73-89,106-157,323-355.
 //
-// Why this form.  The pair-based kernel (sparse_conv_sm90.cu, D3B_ALGO_TC_PAIRS) sums the offsets' partial products
+// Why this form.  A pair-based kernel (spconv's gather -> GEMM -> scatter-add) sums the offsets' partial products
 // with fp32 atomics: summation order -- hence the last bits -- changes run to run, and it needs buffer-clearing launches
 // and a deferred epilogue.  Here one CTA owns 128 output rows and walks the kernel offsets present in the tile
 // (tile_mask); an (offset, 64-channel slice) is one pipeline slot: gather warps copy the 128 input rows (or zeros where

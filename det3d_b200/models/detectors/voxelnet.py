@@ -35,8 +35,8 @@ class _FusedBevMixin:
     """Routes RPN + heads through the det3d_b200 tensor-core kernels.
 
     math = "fp16x3" (default): NHWC split-f16 planes + TMA tensor maps (csrc/bevconv16_sm90.cu), any RPN the
-    reference builds; "tf32x3": the round-1 gather kernel (stride-1 RPN only), which is also where a forward is
-    re-run when a feature leaves the f16 range (`overflow_flag`)."""
+    reference builds; "tf32x3": the output-stationary 3xTF32 gather kernel over a dense rulebook (csrc/sparse_conv_sm90.cu,
+    stride-1 RPN only), which is also where a forward is re-run when a feature leaves the f16 range (`overflow_flag`)."""
     use_fused_bev = True
     math = "fp16x3"
     _bev16 = None

@@ -127,19 +127,6 @@ class Rulebook:
         self.stride = stride
         self.padding = padding
         self._ws = None
-        self.pairs = None             # (pair_in [K,cap], pair_out [K,cap], pair_count [K]) once built
-
-
-def build_pairs(rb):
-    """Compact nbr into per-offset (in_row, out_row) lists for the pair-based kernel (buffers reused)."""
-    if rb.pairs is None:
-        dev = rb.nbr.device
-        rb.pairs = (torch.empty_like(rb.nbr), torch.empty_like(rb.nbr), torch.zeros(rb.k_vol, dtype=torch.int32, device=dev))
-    pin, pout, cnt = rb.pairs
-    st = _lib.lib().d3b_rulebook_pairs(rb.nbr.data_ptr(), rb.out_level.n.data_ptr(), rb.out_level.cap, rb.k_vol,
-                                       pin.data_ptr(), pout.data_ptr(), cnt.data_ptr(), _lib.current_stream())
-    _lib.check(st, "d3b_rulebook_pairs")
-    return rb
 
 
 def conv_out_spatial(spatial, ksize, stride, padding):
@@ -162,22 +149,12 @@ def alloc_subm_rulebook(level, ksize):
     return Rulebook(nbr, tile_mask, ksize, level, level, "subm")
 
 
-def _pair_ptrs(rb, with_pairs):
-    if not with_pairs:
-        return None, None, None
-    if rb.pairs is None:
-        dev = rb.nbr.device
-        rb.pairs = (torch.empty_like(rb.nbr), torch.empty_like(rb.nbr), torch.zeros(rb.k_vol, dtype=torch.int32, device=dev))
-    return tuple(t.data_ptr() for t in rb.pairs)
-
-
-def build_subm_rulebook(rb, with_pairs=False):
+def build_subm_rulebook(rb):
     level = rb.out_level
-    pin, pout, pcnt = _pair_ptrs(rb, with_pairs)
     with _lib.timed("rulebook", kind="subm", k_vol=rb.k_vol):
         st = _lib.lib().d3b_rulebook_subm(
             level.coors.data_ptr(), level.n.data_ptr(), level.cap, C.byref(level.index), _i3(rb.ksize),
-            rb.nbr.data_ptr(), rb.tile_mask.data_ptr(), pin, pout, pcnt, _lib.current_stream(),
+            rb.nbr.data_ptr(), rb.tile_mask.data_ptr(), _lib.current_stream(),
         )
     _lib.check(st, "d3b_rulebook_subm")
     return rb
@@ -203,14 +180,13 @@ def alloc_conv_rulebook(in_level, ksize, stride, padding, out_cap=None):
     return rb
 
 
-def build_conv_rulebook(rb, with_pairs=False):
+def build_conv_rulebook(rb):
     i, o = rb.in_level, rb.out_level
-    pin, pout, pcnt = _pair_ptrs(rb, with_pairs)
     with _lib.timed("rulebook", kind="conv", k_vol=rb.k_vol):
         st = _lib.lib().d3b_rulebook_conv(
             i.coors.data_ptr(), i.n.data_ptr(), i.cap, C.byref(i.index), _i3(rb.ksize), _i3(rb.stride),
             _i3(rb.padding), C.byref(o.index), o.coors.data_ptr(), o.n.data_ptr(), o.cap,
-            rb.nbr.data_ptr(), rb.tile_mask.data_ptr(), pin, pout, pcnt, rb._ws.data_ptr(), rb._ws.numel(),
+            rb.nbr.data_ptr(), rb.tile_mask.data_ptr(), rb._ws.data_ptr(), rb._ws.numel(),
             _lib.current_stream(),
         )
     _lib.check(st, "d3b_rulebook_conv")
@@ -251,41 +227,17 @@ class ConvWeights:
         _lib.check(st, "d3b_conv_pack_weight")
 
 
-_FORCE_ALGO = None
-
-
-def force_algo(algo):
-    """Testing hook: force D3B_ALGO_SIMT / D3B_ALGO_TC for every new ConvWeights (None = auto)."""
-    global _FORCE_ALGO
-    _FORCE_ALGO = algo
-
-
 def tc_supported(c_in, c_out):
     c_in = (int(c_in) + 3) // 4 * 4      # ConvWeights pads C_in to a multiple of 4 for the tensor-core kernels
     return _lib.lib().d3b_conv_packed_weight_floats(c_in, int(c_out), 27) > 0
 
 
 def default_algo(c_in, c_out):
-    if _FORCE_ALGO is not None:
-        return _FORCE_ALGO
     return _lib.ALGO_TC if tc_supported(c_in, c_out) else _lib.ALGO_SIMT
 
 
-def zero_rows(bufs, level):
-    """Clear rows [0, n) of every tensor in `bufs` ([cap, C] f32 sharing `level`'s row count) in one launch."""
-    for i in range(0, len(bufs), 16):
-        chunk = bufs[i:i + 16]
-        ptrs = (C.c_void_p * len(chunk))(*[t.data_ptr() for t in chunk])
-        chans = (C.c_int32 * len(chunk))(*[int(t.shape[1]) for t in chunk])
-        st = _lib.lib().d3b_zero_rows(ptrs, chans, len(chunk), level.n.data_ptr(), level.cap, _lib.current_stream())
-        _lib.check(st, "d3b_zero_rows")
-
-
-def sparse_conv(feat_in, rb, cw, feat_out, residual=None, in_act=None, out_zeroed=False):
-    """feat_out[:n_out] = epilogue(sum_k feat_in[nbr[k]] @ W[k]).  All device-side.
-
-    With cw.algo == ALGO_TC_PAIRS the kernel writes RAW sums (no bias/BN/ReLU/residual of this layer)
-    and `in_act` = (bias, scale, shift, relu) of the producing layer is applied to the gathered inputs."""
+def sparse_conv(feat_in, rb, cw, feat_out, residual=None):
+    """feat_out[:n_out] = epilogue(sum_k feat_in[nbr[k]] @ W[k]).  All device-side."""
     if feat_in.shape[1] == cw.c_in_logical and cw.c_in != cw.c_in_logical:
         feat_in = torch.nn.functional.pad(feat_in, (0, cw.c_in - cw.c_in_logical))
     assert feat_in.dtype == torch.float32 and feat_in.is_contiguous() and feat_in.shape[1] == cw.c_in
@@ -302,17 +254,6 @@ def sparse_conv(feat_in, rb, cw, feat_out, residual=None, in_act=None, out_zeroe
     p.residual = _lib.ptr(residual)
     p.relu = 1 if cw.relu else 0
     p.algo = cw.algo
-    if cw.algo == _lib.ALGO_TC_PAIRS:
-        assert residual is None, "the pair-based kernel defers its epilogue: use feature_epilogue for residuals"
-        if rb.pairs is None:
-            build_pairs(rb)
-        p.pair_in, p.pair_out, p.pair_count = (t.data_ptr() for t in rb.pairs)
-        p.out_zeroed = 1 if out_zeroed else 0
-        if in_act is not None:
-            b, sc, sh, relu = in_act
-            p.in_bias, p.in_scale, p.in_shift, p.in_relu = _lib.ptr(b), _lib.ptr(sc), _lib.ptr(sh), 1 if relu else 0
-    else:
-        assert in_act is None, "only the pair-based kernel applies a deferred input activation"
     dense = rb.kind == "dense2d"
     tag = ("bev3x3" if rb.k_vol == 9 else "bev1x1") if dense else "sparse"
     with _lib.timed(tag, c_in=cw.c_in, c_out=cw.c_out, k_vol=cw.k_vol, math="tf32x3"):
@@ -322,15 +263,6 @@ def sparse_conv(feat_in, rb, cw, feat_out, residual=None, in_act=None, out_zeroe
         )
     _lib.check(st, "d3b_sparse_conv")
     return feat_out
-
-
-def feature_epilogue(feat, level, bias=None, scale=None, shift=None, residual=None, relu=False):
-    """In place over the live rows: x = relu?((x + bias) * scale + shift + residual)."""
-    st = _lib.lib().d3b_feature_epilogue(feat.data_ptr(), level.n.data_ptr(), level.cap, feat.shape[1], _lib.ptr(bias),
-                                         _lib.ptr(scale), _lib.ptr(shift), _lib.ptr(residual), 1 if relu else 0,
-                                         _lib.current_stream())
-    _lib.check(st, "d3b_feature_epilogue")
-    return feat
 
 
 def sparse_to_dense(feat, level, out=None):

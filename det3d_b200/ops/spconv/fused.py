@@ -40,6 +40,28 @@ def _bn_fold(bn):
     return scale.float(), shift.float()
 
 
+def _signature(L):
+    """Identity of the parameters a layer's device weights were made from (version + storage of each tensor)."""
+    tensors = [L.conv.weight, L.conv.bias]
+    if L.bn is not None:
+        tensors += [L.bn.weight, L.bn.bias, L.bn.running_mean, L.bn.running_var]
+    return tuple((None if t is None else (t._version, t.data_ptr())) for t in tensors)
+
+
+def _folded_bn(L, device):
+    """(scale, shift) of the layer's BatchNorm on `device`, or (None, None) without one."""
+    if L.bn is None:
+        return None, None
+    if L.bn.training:
+        raise RuntimeError("det3d_b200 sparse encoders are inference-only: call .eval() first")
+    scale, shift = _bn_fold(L.bn)
+    return scale.to(device), shift.to(device)
+
+
+def _conv_bias(L, device):
+    return None if L.conv.bias is None else L.conv.bias.to(device)
+
+
 def _is_basic_block(m):
     return all(hasattr(m, a) for a in ("conv1", "bn1", "conv2", "bn2", "relu")) and isinstance(
         getattr(m, "conv1"), SparseConvolution
@@ -79,41 +101,23 @@ class FusedSparseEncoder:
     def __init__(self, middle_conv):
         self.plan = compile_plan(middle_conv)
         self._state = None
-        # "fp16x3" (default): output-stationary wgmma kernels on split-f16 planes (csrc/spconv16_sm90.cu) --
-        # deterministic, fused epilogues, no atomics.  "tf32x3": the round-1 kernels (pair-based + fp32 atomics, or
-        # output-stationary with deterministic=True); also the fallback when a feature leaves the f16 range.
+        # "fp16x3" (default): output-stationary wgmma kernels on split-f16 planes (csrc/spconv16_sm90.cu).  "tf32x3":
+        # the output-stationary 3xTF32 kernels (csrc/sparse_conv_sm90.cu, SIMT where the shape is not built), the
+        # fallback when a feature leaves the f16 range.  Both are deterministic: fused epilogues, no atomics.
         self.math = "fp16x3"
         self.external_overflow = None   # int32[1] device flag shared with the rest of the model (else a private one)
         self.algo_override = None  # testing hook (tf32x3 path): force SIMT / TC for every layer
-        # deterministic=True runs every layer output-stationary (D3B_ALGO_TC: one CTA owns an output tile, fixed
-        # summation order, no atomics) -> bit-identical results run to run; the default pair-based kernel sums the
-        # offsets' partial products with fp32 atomics, whose order varies
-        self.deterministic = False
-        self.overlap_rulebooks = True   # build the rulebook chain on a side stream (see run)
+        self.overlap_rulebooks = True   # build the rulebook chain on a side stream (see _fork_rulebooks)
 
     # ---- parameters ------------------------------------------------------------
     def _refresh_weights(self, device):
         for L in self.plan:
-            tensors = [L.conv.weight, L.conv.bias]
-            if L.bn is not None:
-                tensors += [L.bn.weight, L.bn.bias, L.bn.running_mean, L.bn.running_var]
-            sig = tuple((None if t is None else (t._version, t.data_ptr())) for t in tensors) + (self.algo_override, self.deterministic)
+            sig = _signature(L) + (self.algo_override,)
             if L.cw is not None and L.sig == sig:
                 continue
-            if L.bn is not None and L.bn.training:
-                raise RuntimeError("det3d_b200 sparse encoders are inference-only: call .eval() first")
-            scale = shift = None
-            if L.bn is not None:
-                scale, shift = _bn_fold(L.bn)
-                scale, shift = scale.to(device), shift.to(device)
-            algo = self.algo_override
-            if algo is None:   # sparse levels: compacted pairs on the tensor cores whenever the shape allows
-                tc = _lib.ALGO_TC if self.deterministic else _lib.ALGO_TC_PAIRS
-                algo = tc if core.tc_supported(L.conv.in_channels, L.conv.out_channels) else _lib.ALGO_SIMT
-            L.cw = core.ConvWeights(
-                L.conv.weight.to(device), bias=None if L.conv.bias is None else L.conv.bias.to(device),
-                scale=scale, shift=shift, relu=L.relu, algo=algo,
-            )
+            scale, shift = _folded_bn(L, device)
+            L.cw = core.ConvWeights(L.conv.weight.to(device), bias=_conv_bias(L, device), scale=scale, shift=shift,
+                                    relu=L.relu, algo=self.algo_override)
             L.sig = sig
 
     # ---- buffers -----------------------------------------------------------------
@@ -125,7 +129,6 @@ class FusedSparseEncoder:
         st["level0"] = level
         steps = []       # (layer, rulebook, build_fn or None)
         keyed = {}       # (indice_key) -> rulebook
-        pools = {}
         cur = level
         for L in self.plan:
             conv = L.conv
@@ -142,10 +145,9 @@ class FusedSparseEncoder:
                 rb = core.alloc_conv_rulebook(cur, conv.kernel_size, conv.stride, conv.padding)
                 build = core.build_conv_rulebook
                 cur = rb.out_level
-            pools.setdefault((rb.out_level.cap, conv.out_channels), [])
             steps.append((L, rb, build))
         st["steps"] = steps
-        st["pools"] = pools
+        st["pools"] = {}
         st["final_level"] = cur
         c_last = self.plan[-1].conv.out_channels
         d, h, w = cur.spatial
@@ -153,18 +155,67 @@ class FusedSparseEncoder:
         return st
 
     @staticmethod
-    def _wants_pairs(st, rb):
-        return any(M.cw.algo == _lib.ALGO_TC_PAIRS for M, r2, _b in st["steps"] if r2 is rb)
-
-    @staticmethod
-    def _take(pools, cap, c, busy, device):
-        pool = pools[(cap, c)]
+    def _take(pools, key, busy, make):
+        """A buffer of pool `key` that is none of `busy`; make() adds one when all are busy."""
+        pool = pools.setdefault(key, [])
         for t in pool:
             if all(t is not b for b in busy):
                 return t
-        t = torch.empty((max(cap, 1), c), dtype=torch.float32, device=device)
+        t = make()
         pool.append(t)
         return t
+
+    @staticmethod
+    def _adopt_level0(st, features, coors, n_dev):
+        """Take the caller's coordinate rows (and live-row count) as level 0 and index them; returns the fp32 features."""
+        device = features.device
+        m = features.shape[0]
+        lvl0 = st["level0"]
+        coors = coors.to(torch.int32).contiguous()
+        feats = features.to(torch.float32).contiguous()
+        if m == 0:  # keep pointers valid; the device row count (0) makes every kernel a no-op
+            feats = torch.zeros((1, features.shape[1]), dtype=torch.float32, device=device)
+        else:
+            lvl0.coors[:m].copy_(coors)
+        if n_dev is None:
+            lvl0.n.fill_(m)
+        else:
+            lvl0.n[:1].copy_(n_dev.reshape(-1)[:1].to(torch.int32))
+            lvl0.n[1:2].copy_(lvl0.n[:1])
+        lvl0.rebuild_index()
+        return feats
+
+    def _fork_rulebooks(self, st, device):
+        """Rulebooks depend on coordinates only: build the whole chain (level 0 .. 3) on a side stream while the main
+        stream runs the convolutions of the levels already indexed.  Fork / join through events, so the overlap is
+        preserved as parallel branches when the forward is captured into a CUDA graph.
+
+        Returns (side, before_conv): `side` is the side stream, or None when the chain is built in line on the main
+        stream; before_conv(rb, build) is called before each step's convolution."""
+        main = torch.cuda.current_stream(device)
+        builds = [(rb, build) for _L, rb, build in st["steps"] if build is not None]
+        if not (self.overlap_rulebooks and len(builds) > 1):
+            def build_in_line(rb, build):
+                if build is not None:
+                    build(rb)
+            return None, build_in_line
+        side = st.get("side_stream")
+        if side is None:
+            side = st["side_stream"] = torch.cuda.Stream(device=device)
+        side.wait_stream(main)
+        ready = {}
+        with torch.cuda.stream(side):
+            for rb, build in builds:
+                build(rb)
+                ev = torch.cuda.Event()
+                ev.record(side)
+                ready[id(rb)] = ev
+
+        def wait_once(rb, _build):
+            ev = ready.pop(id(rb), None)
+            if ev is not None:
+                main.wait_event(ev)
+        return side, wait_once
 
     # ---- run ------------------------------------------------------------------------
     def run(self, features, coors, batch_size, spatial, n_dev=None, row_cap=None, bev_rows=False):
@@ -189,94 +240,20 @@ class FusedSparseEncoder:
         if bev_rows == "planes":
             raise ValueError("BEV planes are produced by the fp16x3 path only")
         self._refresh_weights(device)
-        lvl0 = st["level0"]
-        # adopt the caller's coordinate rows (zero-copy) for this run
-        coors = coors.to(torch.int32).contiguous()
-        feats = features.to(torch.float32).contiguous()
-        if m == 0:  # keep pointers valid; the device row count (0) makes every kernel a no-op
-            feats = torch.zeros((1, features.shape[1]), dtype=torch.float32, device=device)
-        if m > 0:
-            lvl0.coors[:m].copy_(coors)
-        if n_dev is None:
-            lvl0.n.fill_(m)
-        else:
-            lvl0.n[:1].copy_(n_dev.reshape(-1)[:1].to(torch.int32))
-            lvl0.n[1:2].copy_(lvl0.n[:1])
-        lvl0.rebuild_index()
-
-        x = feats
+        x = self._adopt_level0(st, features, coors, n_dev)
+        _side, before_conv = self._fork_rulebooks(st, device)
         identity = None
-        pending = None   # deferred epilogue (bias, scale, shift, relu) of the layer that produced raw sums in x
-        x_level = lvl0
-
-        def materialize():
-            nonlocal pending
-            if pending is not None:
-                core.feature_epilogue(x, x_level, *pending[:3], relu=pending[3])
-                pending = None
-
-        # Rulebooks depend on coordinates only: build the whole chain (level 0 .. 3) on a side stream while the
-        # main stream runs the convolutions of the levels already indexed.  Fork / join through events, so the
-        # overlap is preserved as parallel branches when the forward is captured into a CUDA graph.
-        main = torch.cuda.current_stream(device)
-        ready = {}
-        planes_cleared = None
-        builds = [(rb, build) for _L, rb, build in st["steps"] if build is not None]
-        # the pair-based kernel accumulates with atomics into a zeroed buffer: one dedicated output buffer per layer,
-        # so that all of a resolution's targets can be cleared up front, off the critical path
-        pair_outs = st.setdefault("pair_outs", {})
-        for i, (L, rb, _b) in enumerate(st["steps"]):
-            if L.cw.algo == _lib.ALGO_TC_PAIRS and i not in pair_outs:
-                pair_outs[i] = torch.empty((max(rb.out_level.cap, 1), L.conv.out_channels), dtype=torch.float32, device=device)
-        is_pairs = [L.cw.algo == _lib.ALGO_TC_PAIRS for L, _r, _b in st["steps"]]
-
-        def prepare(rb, build):
-            build(rb, with_pairs=self._wants_pairs(st, rb))
-            bufs = [pair_outs[i] for i, (_L, r2, _b) in enumerate(st["steps"]) if r2 is rb and is_pairs[i]]
-            if bufs:
-                core.zero_rows(bufs, rb.out_level)
-
-        if self.overlap_rulebooks and len(builds) > 1:
-            side = st.get("side_stream")
-            if side is None:
-                side = st["side_stream"] = torch.cuda.Stream(device=device)
-            side.wait_stream(main)
-            with torch.cuda.stream(side):
-                for rb, build in builds:
-                    prepare(rb, build)
-                    ev = torch.cuda.Event()
-                    ev.record(side)
-                    ready[id(rb)] = ev
-            builds = []
-        waited = set()
-
-        for i, (L, rb, build) in enumerate(st["steps"]):
-            if build is not None and builds:   # single-stream order
-                prepare(rb, build)
-            if id(rb) in ready and id(rb) not in waited:
-                main.wait_event(ready[id(rb)])
-                waited.add(id(rb))
-            pairs = L.cw.algo == _lib.ALGO_TC_PAIRS
+        for L, rb, build in st["steps"]:
+            before_conv(rb, build)
             if L.save_identity:
-                materialize()            # the block input is needed as activated values
                 identity = x
-            if not pairs:
-                materialize()            # output-stationary kernels read activated inputs
-            if pairs:
-                out = pair_outs[i]
-                core.sparse_conv(x, rb, L.cw, out, in_act=pending, out_zeroed=True)
-                pending = (L.cw.bias, L.cw.scale, L.cw.shift, L.cw.relu)
-                x, x_level = out, rb.out_level
-                if L.residual:
-                    core.feature_epilogue(x, x_level, *pending[:3], residual=identity, relu=pending[3])
-                    pending, identity = None, None
-            else:
-                out = self._take(st["pools"], rb.out_level.cap, L.conv.out_channels, (x, identity), device)
-                core.sparse_conv(x, rb, L.cw, out, residual=identity if L.residual else None)
-                if L.residual:
-                    identity = None
-                x, x_level = out, rb.out_level
-        materialize()
+            cap, c = rb.out_level.cap, L.conv.out_channels
+            out = self._take(st["pools"], (cap, c), (x, identity),
+                             lambda: torch.empty((max(cap, 1), c), dtype=torch.float32, device=device))
+            core.sparse_conv(x, rb, L.cw, out, residual=identity if L.residual else None)
+            if L.residual:
+                identity = None
+            x = out
         if bev_rows:
             # channels-last [B*H*W, C*D] with channel = c*D + z: same values as dense.view(B, C*D, H, W)
             d, h, w = st["final_level"].spatial
@@ -294,31 +271,13 @@ class FusedSparseEncoder:
     # ---- FP16x3 path ------------------------------------------------------------------------
     def _refresh_weights16(self, device):
         for L in self.plan:
-            tensors = [L.conv.weight, L.conv.bias]
-            if L.bn is not None:
-                tensors += [L.bn.weight, L.bn.bias, L.bn.running_mean, L.bn.running_var]
-            sig = tuple((None if t is None else (t._version, t.data_ptr())) for t in tensors)
+            sig = _signature(L)
             if L.cw16 is not None and L.sig16 == sig:
                 continue
-            if L.bn is not None and L.bn.training:
-                raise RuntimeError("det3d_b200 sparse encoders are inference-only: call .eval() first")
-            scale = shift = None
-            if L.bn is not None:
-                scale, shift = _bn_fold(L.bn)
-                scale, shift = scale.to(device), shift.to(device)
-            L.cw16 = conv16.ConvWeights16(L.conv.weight.to(device), bias=None if L.conv.bias is None else L.conv.bias.to(device),
-                                          scale=scale, shift=shift, relu=L.relu)
+            scale, shift = _folded_bn(L, device)
+            L.cw16 = conv16.ConvWeights16(L.conv.weight.to(device), bias=_conv_bias(L, device), scale=scale, shift=shift,
+                                          relu=L.relu)
             L.sig16 = sig
-
-    @staticmethod
-    def _take16(pools, cap, c, busy, device):
-        pool = pools.setdefault(("p16", cap, c), [])
-        for t in pool:
-            if all(t is not b for b in busy):
-                return t
-        t = conv16.Planes((max(cap, 1), c), device)
-        pool.append(t)
-        return t
 
     def _bev_planes(self, st, batch_size, device):
         """NHWC f16 planes [B, H, W, C * D] of the encoder output (scn.py:192-195: dense.view(N, C * D, H, W))."""
@@ -343,68 +302,35 @@ class FusedSparseEncoder:
 
     def _run16(self, st, features, coors, batch_size, n_dev, bev_rows):
         device = features.device
-        m = features.shape[0]
         self._refresh_weights16(device)
-        lvl0 = st["level0"]
-        coors = coors.to(torch.int32).contiguous()
-        feats = features.to(torch.float32).contiguous()
-        if m == 0:
-            feats = torch.zeros((1, features.shape[1]), dtype=torch.float32, device=device)
-        if m > 0:
-            lvl0.coors[:m].copy_(coors)
-        if n_dev is None:
-            lvl0.n.fill_(m)
-        else:
-            lvl0.n[:1].copy_(n_dev.reshape(-1)[:1].to(torch.int32))
-            lvl0.n[1:2].copy_(lvl0.n[:1])
-        lvl0.rebuild_index()
+        feats = self._adopt_level0(st, features, coors, n_dev)
         ovf = self.external_overflow
         if ovf is None:
             ovf = st.get("overflow")
             if ovf is None:
                 ovf = st["overflow"] = torch.zeros(1, dtype=torch.int32, device=device)
-
-        # rulebooks depend on coordinates only: the chain of all levels runs on a side stream (fork / join through
-        # events, kept as parallel branches inside a CUDA graph) while the main stream convolves the levels already indexed
-        main = torch.cuda.current_stream(device)
-        ready = {}
-        builds = [(rb, build) for _L, rb, build in st["steps"] if build is not None]
-        if self.overlap_rulebooks and len(builds) > 1:
-            side = st.get("side_stream")
-            if side is None:
-                side = st["side_stream"] = torch.cuda.Stream(device=device)
-            side.wait_stream(main)
+        side, before_conv = self._fork_rulebooks(st, device)
+        planes_cleared = None
+        if bev_rows and side is not None:
+            # the BEV planes are cleared behind the rulebook chain, off the critical path (18 MB for SECOND)
             with torch.cuda.stream(side):
-                for rb, build in builds:
-                    build(rb, with_pairs=False)
-                    ev = torch.cuda.Event()
-                    ev.record(side)
-                    ready[id(rb)] = ev
-                if bev_rows:
-                    # the BEV planes are cleared behind the rulebook chain, off the critical path (18 MB for SECOND)
-                    self._bev_planes(st, batch_size, device).zero_()
-                    planes_cleared = torch.cuda.Event()
-                    planes_cleared.record(side)
-            builds = []
-        waited = set()
+                self._bev_planes(st, batch_size, device).zero_()
+                planes_cleared = torch.cuda.Event()
+                planes_cleared.record(side)
 
         first = self.plan[0].cw16
         x = feats if first.fp32_input else conv16.Planes.from_f32(feats, ovf)
         identity = None
-        x_level = lvl0
         for L, rb, build in st["steps"]:
-            if build is not None and builds:
-                build(rb, with_pairs=False)
-            if id(rb) in ready and id(rb) not in waited:
-                main.wait_event(ready[id(rb)])
-                waited.add(id(rb))
+            before_conv(rb, build)
             if L.save_identity:
                 identity = x
-            out = self._take16(st["pools"], rb.out_level.cap, L.conv.out_channels, (x, identity), device)
+            cap, c = rb.out_level.cap, L.conv.out_channels
+            out = self._take(st["pools"], ("p16", cap, c), (x, identity), lambda: conv16.Planes((max(cap, 1), c), device))
             conv16.sparse_conv16(x, rb, L.cw16, out, residual=identity if L.residual else None, overflow=ovf)
             if L.residual:
                 identity = None
-            x, x_level = out, rb.out_level
+            x = out
         final = st["final_level"]
         d, h, w = final.spatial
         c = x.shape[-1]
@@ -412,7 +338,7 @@ class FusedSparseEncoder:
             planes = self._bev_planes(st, batch_size, device)
             assert tuple(planes.shape) == (batch_size, h, w, c * d)
             if planes_cleared is not None:
-                main.wait_event(planes_cleared)
+                torch.cuda.current_stream(device).wait_event(planes_cleared)
             else:
                 planes.zero_()
             conv16.sparse_to_bev16(x, final, planes)

@@ -181,13 +181,10 @@ size_t d3b_rulebook_workspace_bytes(int64_t n_words);
 int d3b_index_build_hash(const int32_t* coors, const int32_t* n_rows, int32_t row_cap,
                          d3b_site_index* index, void* stream);
 
-/* Submanifold rulebook: outputs == inputs (same rows, same order).
- * pair_in / pair_out [k_vol, row_cap] + pair_count [k_vol] (all three or none, may be NULL): the same
- * map additionally compacted per offset into (in_row, out_row) lists for D3B_ALGO_TC_PAIRS. */
+/* Submanifold rulebook: outputs == inputs (same rows, same order).  Fills nbr and tile_mask. */
 int d3b_rulebook_subm(const int32_t* coors, const int32_t* n_rows, int32_t row_cap,
                       const d3b_site_index* index, const int32_t ksize[3],
-                      int32_t* nbr, uint32_t* tile_mask, int32_t* pair_in, int32_t* pair_out,
-                      int32_t* pair_count, void* stream);
+                      int32_t* nbr, uint32_t* tile_mask, void* stream);
 
 /* Strided sparse conv rulebook.  Output sites = every site reachable from an
  * active input, in ascending linear index ((b*D+z)*H+y)*W+x.  Fills
@@ -196,8 +193,7 @@ int d3b_rulebook_conv(const int32_t* in_coors, const int32_t* n_in, int32_t in_c
                       const d3b_site_index* in_index, const int32_t ksize[3],
                       const int32_t stride[3], const int32_t padding[3],
                       d3b_site_index* out_index, int32_t* out_coors, int32_t* n_out,
-                      int32_t out_cap, int32_t* nbr, uint32_t* tile_mask, int32_t* pair_in,
-                      int32_t* pair_out, int32_t* pair_count, void* workspace,
+                      int32_t out_cap, int32_t* nbr, uint32_t* tile_mask, void* workspace,
                       size_t workspace_bytes, void* stream);
 
 /* ========================================================================= *
@@ -211,8 +207,6 @@ int d3b_rulebook_conv(const int32_t* in_coors, const int32_t* n_in, int32_t in_c
  * ========================================================================= */
 #define D3B_ALGO_SIMT 0     /* fp32 FFMA, output-stationary                              */
 #define D3B_ALGO_TC 1       /* wgmma 3xTF32 (fp32-equivalent), output-stationary tiles    */
-#define D3B_ALGO_TC_PAIRS 2 /* wgmma 3xTF32 over compacted rulebook pairs (per offset:    */
-                            /* dense chunks of 128 valid pairs), fp32 atomics into feat_out */
 
 typedef struct {
   int32_t c_in, c_out, k_vol;    /* k_vol = kd*kh*kw                          */
@@ -223,39 +217,8 @@ typedef struct {
   const float* shift;            /* [c_out] or NULL                           */
   const float* residual;         /* [n_out, c_out] or NULL                    */
   int32_t relu;
-  int32_t algo;
-  /* D3B_ALGO_TC_PAIRS only -------------------------------------------------- */
-  const int32_t* pair_in;        /* [k_vol, out_cap] input row of pair j of offset k (d3b_rulebook_pairs) */
-  const int32_t* pair_out;       /* [k_vol, out_cap] output row                                           */
-  const int32_t* pair_count;     /* [k_vol] pairs per offset (device)                                      */
-  /* epilogue of the PRODUCER layer, applied to the gathered input rows in registers:
-   *   x = relu?((x + in_bias) * in_scale + in_shift); NULL pointers = identity.
-   * The kernel itself adds raw sums into feat_out (which it zeroes first) and applies
-   * nothing else: bias/scale/shift/residual/relu of THIS layer are the consumer's job
-   * (next conv's in_* fields, or d3b_feature_epilogue). */
-  const float* in_bias;
-  const float* in_scale;
-  const float* in_shift;
-  int32_t in_relu;
-  int32_t out_zeroed;            /* nonzero: rows [0, *n_out) of feat_out are already zero (d3b_zero_rows), the
-                                    kernel skips its own clearing launch */
+  int32_t algo;                  /* D3B_ALGO_SIMT or D3B_ALGO_TC; any other value: D3B_ERR_INVALID_ARG */
 } d3b_conv_params;
-
-/* Compact the output-stationary map into per-offset pair lists (spconv's classic rulebook form):
- * for every k, the (in_row, out_row) of each valid nbr[k][o], densely packed; pair_count[k] pairs. */
-int d3b_rulebook_pairs(const int32_t* nbr, const int32_t* n_out, int32_t out_cap, int32_t k_vol,
-                       int32_t* pair_in, int32_t* pair_out, int32_t* pair_count, void* stream);
-
-/* Clear rows [0, *n_rows) of up to 16 feature buffers that share a row count, in one launch (the accumulation
- * targets of the D3B_ALGO_TC_PAIRS layers of one resolution).  bufs / channels are HOST arrays of `count` entries;
- * channels[i] % 4 == 0. */
-int d3b_zero_rows(float* const* bufs, const int32_t* channels, int32_t count, const int32_t* n_rows,
-                  int32_t row_cap, void* stream);
-
-/* In-place epilogue over rows [0, *n_rows): x = relu?((x + bias) * scale + shift + residual). */
-int d3b_feature_epilogue(float* feat, const int32_t* n_rows, int32_t row_cap, int32_t channels,
-                         const float* bias, const float* scale, const float* shift,
-                         const float* residual, int32_t relu, void* stream);
 
 /* Size in floats / fill of the tensor-core weight image (hi/lo TF32 split,
  * K-major 128B-swizzled tiles).  Done once per layer at model load. */

@@ -56,10 +56,13 @@ def test_every_plane_writer_takes_an_overflow_flag():
     assert not missing, "write f16 planes without an overflow flag: %s" % missing
 
 
-def test_abi_version_and_error_string():
-    """ABI 3: d3b_sparse_to_bev16 takes the f16-range `overflow` flag (one argument more than in ABI 2)."""
+def test_abi_4_and_error_string():
+    """ABI 4: the rulebook builders no longer take pair lists (three arguments fewer than in ABI 3), and
+    d3b_conv_params lost its pair-kernel fields."""
     L = _lib.lib()
-    assert L.d3b_abi_version() == 3
+    assert L.d3b_abi_version() == 4
+    assert len(_lib.SIGNATURES["d3b_rulebook_subm"][1]) == 8
+    assert len(_lib.SIGNATURES["d3b_rulebook_conv"][1]) == 16
     assert isinstance(L.d3b_last_error(), bytes)
     assert L.d3b_launch_count() >= 0
 
@@ -75,14 +78,24 @@ def test_argument_validation_without_gpu():
     assert st == 1
 
 
-def test_more_argument_validation_without_gpu():
+def test_sparse_conv_rejects_an_unknown_algo_without_gpu():
+    """Only D3B_ALGO_SIMT (0) and D3B_ALGO_TC (1) exist: any other value is an invalid argument, never a silent fall
+    through to another kernel."""
+    L = _lib.lib()
+    dummy = (ctypes.c_float * 16)()
+    for algo in (2, 3, -1):
+        p = _lib.ConvParams(c_in=16, c_out=16, k_vol=27, weight=ctypes.addressof(dummy),
+                            weight_packed=ctypes.addressof(dummy), relu=1, algo=algo)
+        st = L.d3b_sparse_conv(dummy, dummy, dummy, dummy, 128, ctypes.byref(p), dummy, None)
+        assert st == 1 and b"algo" in L.d3b_last_error()
+
+
+def test_entry_points_validate_before_cuda_without_gpu():
     """Every entry point validates before it touches CUDA: status 1 (invalid argument) / 3 (unsupported) + message."""
     L = _lib.lib()
     i3 = (ctypes.c_int32 * 3)(3, 3, 3)
-    assert L.d3b_rulebook_subm(None, None, 10, None, i3, None, None, None, None, None, None) == 1
-    assert L.d3b_rulebook_pairs(None, None, 10, 27, None, None, None, None) == 1
-    assert L.d3b_zero_rows(None, None, 17, None, 10, None) == 1 and b"count" in L.d3b_last_error()
-    assert L.d3b_zero_rows(None, None, 0, None, 10, None) == 0                 # nothing to do
+    assert L.d3b_rulebook_subm(None, None, 10, None, i3, None, None, None) == 1
+    assert L.d3b_rulebook_conv(None, None, 10, None, i3, i3, i3, None, None, None, 10, None, None, None, 0, None) == 1
     assert L.d3b_rotate_nms(None, 10, None, 7, 0.5, 10, None, (ctypes.c_int32 * 1)(), None, 0, None) == 1
     assert b"format" in L.d3b_last_error()
     assert L.d3b_normal_nms(None, 10, None, 5, 0.5, 10, None, (ctypes.c_int32 * 1)(), None, 0, None) == 1

@@ -661,21 +661,20 @@ def tf32x3_bound(algo, c_in, k_vol):
     """|got - y| <= c M for the tf32x3 kernels.  Representation: hi = x with the low 13 mantissa bits cleared, lo = x - hi
     (|lo| < 2^-10 |x|) read by the tensor core as tf32 (error < 2^-10 |lo|), lo.lo dropped: 3 2^-20 M.  Accumulation:
     the output-stationary kernel chains every MMA of the layer (3 per k8 step, C_in / 8 steps per offset, k_vol offsets)
-    into one uncorrected accumulator, each truncation < 2 ulp of the running magnitude <= M: 2 n 2^-23 M; the pair
-    kernel chains one offset's MMAs and adds the k_vol partials with fp32 atomics (u each).  SIMT: one fp32 FMA chain of
-    k_vol C_in terms."""
+    into one uncorrected accumulator, each truncation < 2 ulp of the running magnitude <= M: 2 n 2^-23 M.  SIMT: one
+    fp32 FMA chain of k_vol C_in terms."""
     c4 = (c_in + 3) // 4 * 4
     if algo == "simt":
         L = k_vol * c_in + 2
         return L * U * (1 + L * U)
     n = 3 * ((c4 + 7) // 8) * k_vol
-    return 3 * 2.0 ** -20 + 2 * n * 2.0 ** -23 + (k_vol * U if algo == "pairs" else 0.0)
+    return 3 * 2.0 ** -20 + 2 * n * 2.0 ** -23
 
 
-@pytest.mark.parametrize("algo", ["simt", "tc", "pairs"])
-@pytest.mark.parametrize("c_in,c_out", [(16, 32), (64, 64), (128, 128)])
-def test_tf32x3_sparse_beyond_f16_range(algo, c_in, c_out):
-    """Features around 3e5 (they trip the FP16x3 flag): simt, tc and pairs against the exact y."""
+@pytest.mark.parametrize("algo", ["simt", "tc"])
+@pytest.mark.parametrize("c_in,c_out", [(16, 32), (64, 64), (128, 128), (32, 32), (64, 128)])
+def test_tf32x3_output_stationary_beyond_f16_range(algo, c_in, c_out):
+    """Features around 3e5 (they trip the FP16x3 flag): simt and tc against the exact y, at the encoders' layer shapes."""
     from det3d_b200 import _lib
     from det3d_b200.ops.spconv import conv16, core
     gen = torch.Generator(device="cuda").manual_seed(c_in + c_out)
@@ -686,8 +685,7 @@ def test_tf32x3_sparse_beyond_f16_range(algo, c_in, c_out):
     flag = torch.zeros(1, dtype=torch.int32, device="cuda")
     conv16.Planes.from_f32(x, flag)
     assert int(flag.item()) == 1, "these features must be beyond the FP16x3 range"
-    algo_id = {"simt": _lib.ALGO_SIMT, "tc": _lib.ALGO_TC, "pairs": _lib.ALGO_TC_PAIRS}[algo]
-    cw = core.ConvWeights(w, algo=algo_id)
+    cw = core.ConvWeights(w, algo=_lib.ALGO_SIMT if algo == "simt" else _lib.ALGO_TC)
     out = torch.full((n, c_out), float("nan"), device="cuda")
     core.sparse_conv(x, rb, cw, out)
     idx = rb.nbr[:, :n].long()

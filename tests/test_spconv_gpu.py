@@ -74,12 +74,12 @@ def test_conv_rulebook_overflow_is_reported():
     assert np.array_equal(rb.out_level.coors[:50].cpu().numpy(), want_coors[:50])
 
 
-ALGOS = ["simt", "tc", "pairs"]
+ALGOS = ["simt", "tc"]
 
 
 def _algo(name):
     from det3d_b200 import _lib
-    return {"simt": _lib.ALGO_SIMT, "tc": _lib.ALGO_TC, "pairs": _lib.ALGO_TC_PAIRS}[name]
+    return {"simt": _lib.ALGO_SIMT, "tc": _lib.ALGO_TC}[name]
 
 
 @pytest.mark.parametrize("algo", ALGOS)
@@ -87,8 +87,11 @@ def _algo(name):
     (4, 16, 3, 1, 1, True), (5, 16, 3, 1, 1, True), (16, 16, 3, 1, 1, True), (16, 32, 3, 2, 1, False),
     (32, 32, 3, 1, 1, True), (32, 64, 3, 2, 1, False), (64, 64, 3, 1, 1, True), (64, 64, 3, 2, [0, 1, 1], False),
     (64, 128, 3, 2, [0, 1, 1], False), (128, 128, 3, 1, 1, True), (64, 64, (3, 1, 1), (2, 1, 1), 0, False),
-    (128, 128, (3, 1, 1), (2, 1, 1), 0, False)])
-def test_single_layer_vs_oracle(algo, cin, cout, k, s, p, subm):
+    (128, 128, (3, 1, 1), (2, 1, 1), 0, False),
+    # partial and odd 32-channel slots, C_out < C_in, k_vol 1 and 9
+    (48, 32, 3, 1, 1, True), (96, 128, 3, 1, 1, True), (128, 64, 3, 1, 1, True), (32, 16, 3, 2, 1, False),
+    (64, 64, 1, 1, 0, True), (16, 32, (1, 3, 3), 1, 0, True)])
+def test_output_stationary_layer_vs_oracle(algo, cin, cout, k, s, p, subm):
     from det3d_b200.ops.spconv import core
     if algo != "simt" and not core.tc_supported(cin, cout):
         pytest.skip("tensor-core kernels do not take C_in=%d" % cin)
@@ -116,12 +119,7 @@ def test_single_layer_vs_oracle(algo, cin, cout, k, s, p, subm):
     out = torch.full((rb.out_level.cap, cout), float("nan"), device="cuda")
     res_dev = torch.zeros((rb.out_level.cap, cout), device="cuda")
     res_dev[:n_out] = torch.from_numpy(res).cuda()
-    if algo == "pairs":
-        # raw sums, then the layer's epilogue as a separate pass (what a consumer / d3b_feature_epilogue does)
-        core.sparse_conv(torch.from_numpy(feat).cuda(), rb, cw, out)
-        core.feature_epilogue(out, rb.out_level, cw.bias, cw.scale, cw.shift, residual=res_dev, relu=True)
-    else:
-        core.sparse_conv(torch.from_numpy(feat).cuda(), rb, cw, out, residual=res_dev)
+    core.sparse_conv(torch.from_numpy(feat).cuda(), rb, cw, out, residual=res_dev)
     want = torch.relu((osp.indice_conv(feat, w, nbr, n_out, bias) * torch.from_numpy(scale) + torch.from_numpy(shift))
                       + torch.from_numpy(res))
     got = out[:n_out].cpu()
@@ -188,29 +186,3 @@ def test_dense_matches_oracle():
     feat = rng.standard_normal((700, 64)).astype(np.float32)
     t = SparseConvTensor(torch.from_numpy(feat).cuda(), torch.from_numpy(coors).cuda(), spatial, batch)
     assert torch.equal(t.dense().cpu(), osp.dense(feat, coors, spatial, batch))
-
-
-def test_pairs_kernel_deferred_input_activation():
-    """Two chained pair-based layers: layer 2 applies layer 1's bias/BN/ReLU while gathering."""
-    from det3d_b200 import _lib
-    from det3d_b200.ops.spconv import core
-    rng = np.random.default_rng(9)
-    spatial, batch, n = (11, 40, 36), 2, 4000
-    coors = _sites(rng, n, spatial, batch)
-    feat = rng.standard_normal((n, 16)).astype(np.float32)
-    w1 = (rng.standard_normal((3, 3, 3, 16, 32)) * 0.1).astype(np.float32)
-    w2 = (rng.standard_normal((3, 3, 3, 32, 64)) * 0.1).astype(np.float32)
-    b1, s1, t1 = (rng.standard_normal(32).astype(np.float32) for _ in range(3))
-    lvl = core.level_from_coors(torch.from_numpy(coors).cuda(), spatial, batch)
-    rb = core.build_subm_rulebook(core.alloc_subm_rulebook(lvl, 3))
-    g = lambda a: torch.from_numpy(a).cuda()
-    cw1 = core.ConvWeights(g(w1), bias=g(b1), scale=g(s1), shift=g(t1), relu=True, algo=_lib.ALGO_TC_PAIRS)
-    cw2 = core.ConvWeights(g(w2), algo=_lib.ALGO_TC_PAIRS)
-    y1 = torch.empty((n, 32), device="cuda")
-    y2 = torch.empty((n, 64), device="cuda")
-    core.sparse_conv(g(feat), rb, cw1, y1)
-    core.sparse_conv(y1, rb, cw2, y2, in_act=(cw1.bias, cw1.scale, cw1.shift, True))
-    nbr = osp.subm_neighbours(coors, spatial, 3)
-    h = torch.relu(osp.indice_conv(feat, w1, nbr, n, b1) * torch.from_numpy(s1) + torch.from_numpy(t1))
-    want = osp.indice_conv(h.numpy(), w2, nbr, n)
-    assert float((y2.cpu() - want).abs().max()) <= TOL * max(1.0, float(want.abs().max()))

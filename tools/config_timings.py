@@ -65,7 +65,8 @@ def main():
     off = [35000 * i for i in range(5)]
     ms = timed(lambda: pipe.pack(pipe.forward_device(p4, off)), iters=5)
     rows.append(("C4 CBGS nuScenes (SpMiddleResNetFHD, 6 task heads), 4 x 35k lidar-like points per GPU", "%.2f ms / batch = %.0f clouds/s per GPU" % (ms, 4e3 / ms),
-                 "21 sparse convs on the pair kernel; strided RPN2 on cuDNN fp32; eager launches"))
+                 "21 sparse convs on the FP16x3 kernels (spconv_first16_kernel for the 5-channel input layer, "
+                 "spconv_os16_kernel for the other 20); strided RPN2 on cuDNN fp32; eager launches"))
     del pipe, model
 
     # C5: rotated NMS stress, 100k boxes

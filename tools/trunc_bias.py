@@ -10,7 +10,7 @@ is printed with its standard error, in units of eps = 2^-26 (kTruncLossPerMma in
 (sparse output-stationary, dense pixel-stationary and pipelined) are measured against the split-exact result yh of the
 operands they see (tests/test_conv_error_model_gpu.py): each full slot chains n = 12 truncating MMAs and the epilogue
 adds 12 eps (kTruncLossPerMma per MMA) to the sums, so the true mean loss per MMA is about (12 eps - beta) / 12.  The tf32x3
-fallback kernels (simt, tc, pairs; tc over a dense rulebook) are measured against the exact y at features ~3e5.
+fallback kernels (simt, tc; tc over a dense rulebook) are measured against the exact y at features ~3e5.
 
     python tools/trunc_bias.py [--out FILE]
 """
@@ -54,9 +54,8 @@ def tf32_case(algo, regime):
     lvl = em._level(n, (20, 100, 100), 2, 11)
     rb = core.build_subm_rulebook(core.alloc_subm_rulebook(lvl, 3))
     x, w = em.operands((n, c), (27, c, c), regime, gen, a_scale=3.0e5)
-    algo_id = {"simt": _lib.ALGO_SIMT, "tc": _lib.ALGO_TC, "pairs": _lib.ALGO_TC_PAIRS}[algo]
     out = torch.empty((n, c), device="cuda")
-    core.sparse_conv(x, rb, core.ConvWeights(w, algo=algo_id), out)
+    core.sparse_conv(x, rb, core.ConvWeights(w, algo=_lib.ALGO_SIMT if algo == "simt" else _lib.ALGO_TC), out)
     idx = rb.nbr[:, :n].long()
     y = torch.zeros((n, c), dtype=torch.float64, device="cuda")
     for k in range(27):
@@ -83,7 +82,7 @@ def main():
             applied = 12 * eps
             rows.append(dict(kernel=kernel, math="fp16x3", regime=regime, outputs=got.numel(), beta_eps=beta / eps,
                              se_eps=se / eps, applied_eps=applied / eps, loss_per_mma_eps=(applied - beta) / 12 / eps))
-    for algo in ("simt", "tc", "pairs", "tc_dense"):
+    for algo in ("simt", "tc", "tc_dense"):
         for regime in ("A", "B", "C"):
             got, y = tf32_case(algo, regime)
             beta, se = em.residual_slope(got, y)
