@@ -72,6 +72,7 @@ class Conv16Params(C.Structure):
         ("bias", C.c_void_p), ("scale", C.c_void_p), ("shift", C.c_void_p),
         ("residual_hi", C.c_void_p), ("residual_lo", C.c_void_p), ("relu", C.c_int32),
         ("out_hi", C.c_void_p), ("out_lo", C.c_void_p), ("out_f32", C.c_void_p), ("overflow", C.c_void_p),
+        ("in_f32_ld", C.c_int32),
     ]
 
 

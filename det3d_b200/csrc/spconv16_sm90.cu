@@ -378,7 +378,7 @@ spconv_os16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ 
 template <int COUT>
 __global__ void __launch_bounds__(256)
 spconv_first16_kernel(const float* __restrict__ feat_in, const int* __restrict__ nbr, const int* __restrict__ n_out_p,
-                      int out_cap, int c_in, int k_vol, const float* __restrict__ weight, Epi16 epi,
+                      int out_cap, int c_in, int in_ld, int k_vol, const float* __restrict__ weight, Epi16 epi,
                       __half* __restrict__ out_hi, __half* __restrict__ out_lo, float* __restrict__ out_f32,
                       int* __restrict__ overflow) {
   extern __shared__ float w_s[];                 // [k_vol][c_in][COUT]
@@ -410,7 +410,7 @@ spconv_first16_kernel(const float* __restrict__ feat_in, const int* __restrict__
       if (src[t] < 0) continue;
       const int k = sub + t * kSub;
       for (int ci = 0; ci < c_in; ++ci) {
-        const float a = __ldg(feat_in + (size_t)src[t] * c_in + ci);
+        const float a = __ldg(feat_in + (size_t)src[t] * in_ld + ci);
         const float* w = w_s + ((size_t)k * c_in + ci) * COUT + col;
 #pragma unroll
         for (int q = 0; q < 16; ++q) acc[q] = fmaf(a, w[q], acc[q]);
@@ -546,7 +546,8 @@ static int launch_first16(const d3b_conv16_params* p, const int32_t* nbr, const 
   D3B_REQUIRE(smem <= 160 * 1024, "first-layer sparse conv: weights (%zu bytes) do not fit in shared memory", smem);
   D3B_CUDA(ensure_dynamic_smem(spconv_first16_kernel<COUT>, smem, optin));
   const int grid = grid_for((long long)out_cap * (COUT / 16) * 4, 256, 8);
-  spconv_first16_kernel<COUT><<<grid, 256, smem, stream>>>(p->in_f32, nbr, n_out, out_cap, p->c_in, p->k_vol, p->weight,
+  const int in_ld = p->in_f32_ld ? p->in_f32_ld : p->c_in;
+  spconv_first16_kernel<COUT><<<grid, 256, smem, stream>>>(p->in_f32, nbr, n_out, out_cap, p->c_in, in_ld, p->k_vol, p->weight,
                                                          epi_of(p), (__half*)p->out_hi, (__half*)p->out_lo, p->out_f32,
                                                          p->overflow);
   D3B_LAUNCH_CHECK();
@@ -595,6 +596,8 @@ extern "C" int d3b_sparse_conv16(const int32_t* nbr, const uint32_t* tile_mask, 
   if (out_cap == 0) return D3B_OK;
   if (p->in_f32) {      // first layer: fp32 rows, few channels
     D3B_REQUIRE(p->weight && p->c_in >= 1 && p->c_in <= 16, "d3b_sparse_conv16: fp32-input layers need weight and C_in <= 16");
+    D3B_REQUIRE(p->in_f32_ld == 0 || p->in_f32_ld >= p->c_in, "d3b_sparse_conv16: in_f32_ld %d < C_in %d", p->in_f32_ld,
+                p->c_in);
     switch (p->c_out) {
       case 16: return launch_first16<16>(p, nbr, n_out, out_cap, stream);
       case 32: return launch_first16<32>(p, nbr, n_out, out_cap, stream);

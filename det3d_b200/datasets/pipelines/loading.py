@@ -3,7 +3,8 @@ and `__call__(res, info)` contract (det3d/datasets/pipelines/loading.py:67-124),
 on the GPU by d3b_ingest_sweeps (csrc/ingest.cu).
 
 File reading stays on the host (it is I/O): KITTI `.bin` = flat float32 [N, num_point_features] (:92-94), nuScenes
-`.pcd.bin` = float32 [N, 5] of which the first 4 columns are kept (`read_file`, :17-31).  Everything after that --
+and Lyft `.bin` = float32 [N, 5] of which the first 4 columns are kept (`read_file`, :17-31; Lyft reads the
+LIDAR_TOP file of `info["ref_info"]`, :128-158, and has no sweeps).  Everything after that --
 the 1 m `remove_close` filter of the sweeps (:34-43), the float64 rigid transform (:55-58), the time-lag column and
 the concatenation (:115-124) -- is one call over the raw bytes of all sweeps.  `res["lidar"]` receives the same
 numpy fields as the reference (`points`, `times`, `combined`) plus `combined_cuda`, the device tensor the
@@ -367,6 +368,10 @@ class LoadPointCloudFromFile(object):
             res["lidar"]["times"] = host[:, 4:5]
             res["lidar"]["combined"] = host
             res["lidar"]["combined_cuda"] = combined
+        elif self.type == "LyftDataset":
+            # loading.py:128-158: the top lidar only (the side-lidar merge there is commented out); read_file keeps
+            # x, y, z, intensity of each 5-float record and drops a trailing partial record
+            res["lidar"]["points"] = read_file(info["ref_info"]["LIDAR_TOP"]["lidar_path"])
         else:
             raise NotImplementedError("LoadPointCloudFromFile: dataset type %s" % self.type)
         return res, info

@@ -16,7 +16,8 @@ class VoxelFeatureExtractorV3(nn.Module):
     def forward(self, features, num_voxels, coors=None):
         c = self.num_input_features
         if features.dim() == 2:
-            # fused path: the voxelizer already produced the per-voxel mean [M, C]
-            return features[:, :c].contiguous()
+            # fused path: the voxelizer already produced the per-voxel mean [M, ndim]; the leading c columns are returned
+            # as a strided view (no copy launch), which the encoder's first layer reads in place
+            return features[:, :c]
         total = features[:, :, :c].sum(dim=1, keepdim=False)
         return (total / num_voxels.type_as(features).view(-1, 1)).contiguous()

@@ -117,14 +117,16 @@ class ConvWeights16:
 
 
 def sparse_conv16(x, rb, cw, out, residual=None, out_f32=None, overflow=None, tag="sparse"):
-    """out[:n_out] = epilogue(sum_k x[nbr[k]] @ W[k]).  x: Planes (or an fp32 [rows, C] tensor for the first layer);
-    out: Planes [cap, C_out] (or None when only `out_f32` is wanted)."""
+    """out[:n_out] = epilogue(sum_k x[nbr[k]] @ W[k]).  x: Planes (or an fp32 [rows, C] tensor for the first layer, whose
+    rows may be strided: a column slice x[:, :C] of wider rows is read in place); out: Planes [cap, C_out] (or None when
+    only `out_f32` is wanted)."""
     p = Conv16Params()
     p.c_in, p.c_out, p.k_vol = cw.c_in, cw.c_out, cw.k_vol
     assert rb.k_vol == cw.k_vol, "kernel volume mismatch"
     if cw.fp32_input:
-        assert torch.is_tensor(x) and x.dtype == torch.float32 and x.is_contiguous() and x.shape[1] == cw.c_in
-        p.in_f32, p.weight = x.data_ptr(), cw.weight.data_ptr()
+        assert torch.is_tensor(x) and x.dtype == torch.float32 and x.dim() == 2 and x.shape[1] == cw.c_in
+        assert x.stride(1) == 1 and x.stride(0) >= cw.c_in, "first-layer rows must have unit column stride"
+        p.in_f32, p.weight, p.in_f32_ld = x.data_ptr(), cw.weight.data_ptr(), x.stride(0)
         dev_t = x
     else:
         assert isinstance(x, Planes) and x.shape[-1] == cw.c_in

@@ -167,12 +167,15 @@ class FusedSparseEncoder:
 
     @staticmethod
     def _adopt_level0(st, features, coors, n_dev):
-        """Take the caller's coordinate rows (and live-row count) as level 0 and index them; returns the fp32 features."""
+        """Take the caller's coordinate rows (and live-row count) as level 0 and index them; returns the fp32 features,
+        which keep their row stride when their columns are contiguous (the FP16x3 first layer reads strided rows)."""
         device = features.device
         m = features.shape[0]
         lvl0 = st["level0"]
         coors = coors.to(torch.int32).contiguous()
-        feats = features.to(torch.float32).contiguous()
+        feats = features.to(torch.float32)
+        if feats.stride(-1) != 1:
+            feats = feats.contiguous()
         if m == 0:  # keep pointers valid; the device row count (0) makes every kernel a no-op
             feats = torch.zeros((1, features.shape[1]), dtype=torch.float32, device=device)
         else:
@@ -240,7 +243,7 @@ class FusedSparseEncoder:
         if bev_rows == "planes":
             raise ValueError("BEV planes are produced by the fp16x3 path only")
         self._refresh_weights(device)
-        x = self._adopt_level0(st, features, coors, n_dev)
+        x = self._adopt_level0(st, features, coors, n_dev).contiguous()
         _side, before_conv = self._fork_rulebooks(st, device)
         identity = None
         for L, rb, build in st["steps"]:

@@ -212,7 +212,9 @@ def calibrate_demo_weights_(model, cfg, clouds, seed=0, pass_fraction=0.03, box_
                 feats = model.reader.forward_torch(out["voxels"][:m_rows], out["num_points"][:m_rows], coors)
                 x = model.backbone(feats.reshape(m_rows, -1), coors, batch, grid)
             else:
-                x = model.backbone.forward_unfused(out["mean"][:m_rows].clone(), coors, batch, grid)
+                # the reader's leading columns (Lyft: 3 of the 4 point columns)
+                c = int(cfg.model["reader"].get("num_input_features", out["mean"].shape[1]))
+                x = model.backbone.forward_unfused(out["mean"][:m_rows, :c].clone(), coors, batch, grid)
             if getattr(model, "with_neck", False):
                 x = model.neck(x)
             thr = float(cfg.test_cfg["score_threshold"])

@@ -303,6 +303,8 @@ typedef struct {
   void* out_lo;
   float* out_f32;                /* optional fp32 copy of the result [rows, c_out]                              */
   int32_t* overflow;             /* device flag, may be NULL                                                    */
+  int32_t in_f32_ld;             /* row stride of in_f32 in floats (>= c_in), 0 = c_in: the first layer can read the
+                                    leading c_in columns of wider rows, e.g. 3 of the voxelizer's 4-column means    */
 } d3b_conv16_params;
 
 /* Size in halves / fill of the f16 weight image: packed[k][kb][hi|lo][n][64 channels, 128B-swizzled].
