@@ -18,6 +18,7 @@ AA_IOU3D, AA_PIXEL = 0, 1
 BOX_XYXYR = 0
 BOX_XYWLR = 1
 BOX_XYWLR_RRPN = 2
+IOU_BEV_XYXYR, OVERLAP_BEV_XYXYR, IOU_BEV_XYWLR = 0, 1, 2     # d3b_boxes_iou_bev modes
 
 
 class D3BError(RuntimeError):

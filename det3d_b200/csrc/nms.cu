@@ -261,9 +261,18 @@ __device__ __forceinline__ float standup_iou(const Quad& a, const Quad& b) {
   return __fdiv_rn(inter, ua);
 }
 
+// Vertex capacity of the clipper.  In exact arithmetic clipping a convex polygon by a half-plane adds at most one vertex,
+// so the four steps never exceed 8.  In floating point the near-duplicate pairs NMS sees all the time (the same box one
+// ulp or 1e-9 rad apart) make the sign tests of a clip step disagree with the geometry: the rounded polygon is not convex
+// any more, and a clip step can meet more than two sign changes (more than 8 vertices).  The bound that holds for
+// any sign pattern: one step keeps the k vertices with d >= 0 and adds one per sign change of the cyclic sequence of n
+// vertices, and there are at most 2 * min(k, n - k) of those, so m <= k + 2 min(k, n - k) <= floor(3n / 2).  From 4
+// corners: 6, 9, 13, 19.
+constexpr int kClipMaxVertices = 19;
+
 // Convex quad ∩ convex quad by Sutherland-Hodgman in fp64; returns area.
 __device__ double quad_intersection_area(const Quad& A, const Quad& B) {
-  double px[10], py[10], qx[10], qy[10];
+  double px[kClipMaxVertices], py[kClipMaxVertices], qx[kClipMaxVertices], qy[kClipMaxVertices];
   int n = 4;
   for (int k = 0; k < 4; ++k) { px[k] = A.x[k]; py[k] = A.y[k]; }
   // orientation of the clip polygon
@@ -311,25 +320,15 @@ __device__ __forceinline__ double quad_area(const Quad& q) {
 }
 
 // nms_cpu.h:103-158: skip unless hulls overlap; overlap = inter / union; suppress when >= thresh.
-// the polygon part of the test, for a pair whose hulls overlap (standup_iou > 0)
-__device__ __forceinline__ bool clip_suppresses_xywlr(const Quad& a, const Quad& b, float thresh) {
+// The rotate_nms_cc IoU of a pair whose hulls overlap (standup_iou > 0; the caller applies that gate).  NaN when the
+// pair is skipped (empty intersection -- boost's empty output -- or empty union): no threshold suppresses it, where an
+// IoU of 0 would be suppressed at threshold 0.  The NMS mask and the mode-2 IoU matrix both call this.
+__device__ __forceinline__ float clip_iou_xywlr(const Quad& a, const Quad& b) {
   const double inter = quad_intersection_area(a, b);
-  if (!(inter > 0.0)) return false;
+  if (!(inter > 0.0)) return __int_as_float(0x7fffffff);
   const double uni = quad_area(a) + quad_area(b) - inter;
-  if (!(uni > 0.0)) return false;
-  return (float)(inter / uni) >= thresh;
-}
-
-__device__ __forceinline__ bool suppresses_xywlr(const Quad& a, const Quad& b, float thresh, float* iou_out) {
-  if (iou_out) *iou_out = 0.0f;
-  if (standup_iou(a, b) <= 0.0f) return false;
-  const double inter = quad_intersection_area(a, b);
-  if (!(inter > 0.0)) return false;  // boost: empty intersection output -> nothing to test
-  const double uni = quad_area(a) + quad_area(b) - inter;
-  if (!(uni > 0.0)) return false;
-  const float ov = (float)(inter / uni);
-  if (iou_out) *iou_out = ov;
-  return ov >= thresh;
+  if (!(uni > 0.0)) return __int_as_float(0x7fffffff);
+  return (float)(inter / uni);
 }
 
 
@@ -473,7 +472,18 @@ pair_matrix_kernel(int na, const float* __restrict__ boxes_a, int nb, const floa
   if (a >= na || b >= nb) return;
   const float* pa = boxes_a + (size_t)a * 5;
   const float* pb = boxes_b + (size_t)b * 5;
-  out[(size_t)a * nb + b] = MODE == 0 ? iou_xyxyr(pa, pb) : overlap_xyxyr(pa, pb);
+  if constexpr (MODE == 2) {
+    // rotate_nms_cc overlap: 0 for a pair the hull gate or the polygon test skips
+    const Quad qa = quad_of_xywlr(pa), qb = quad_of_xywlr(pb);
+    float v = 0.0f;
+    if (standup_iou(qa, qb) > 0.0f) {
+      v = clip_iou_xywlr(qa, qb);
+      if (v != v) v = 0.0f;
+    }
+    out[(size_t)a * nb + b] = v;
+  } else {
+    out[(size_t)a * nb + b] = MODE == 0 ? iou_xyxyr(pa, pb) : overlap_xyxyr(pa, pb);
+  }
 }
 
 // Suppression bitmask, upper triangle only.  A work item is (64-box row block, 64-box column
@@ -582,7 +592,7 @@ nms_mask_kernel(const float* __restrict__ boxes, int n_cap, const int* __restric
       const int n_pairs = s_count;
       for (int e = threadIdx.x; e < n_pairs; e += blockDim.x) {
         const int rr = s_list[e] >> 6, cc = s_list[e] & 63;
-        if (clip_suppresses_xywlr(qrow[rr], qcol[cc], thresh)) atomicOr(&s_bits[rr * 2 + (cc >> 5)], 1u << (cc & 31));
+        if (clip_iou_xywlr(qrow[rr], qcol[cc]) >= thresh) atomicOr(&s_bits[rr * 2 + (cc >> 5)], 1u << (cc & 31));
       }
       __syncthreads();
       if (threadIdx.x < 2 * kNmsRowsPerCta) {
@@ -805,14 +815,16 @@ using namespace d3b;
 extern "C" int d3b_boxes_iou_bev(const float* boxes_a, int32_t na, const float* boxes_b, int32_t nb,
                                  int32_t mode, float* out, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  D3B_REQUIRE(na >= 0 && nb >= 0 && (mode == 0 || mode == 1), "d3b_boxes_iou_bev: bad argument");
+  D3B_REQUIRE(na >= 0 && nb >= 0 && mode >= 0 && mode <= 2, "d3b_boxes_iou_bev: bad argument (mode %d)", mode);
   if (na == 0 || nb == 0) return D3B_OK;
   D3B_REQUIRE(boxes_a && boxes_b && out, "d3b_boxes_iou_bev: null argument");
   dim3 blocks(div_up(nb, 16), div_up(na, 16)), threads(16, 16);
   if (mode == 0)
     pair_matrix_kernel<0><<<blocks, threads, 0, stream>>>(na, boxes_a, nb, boxes_b, out);
-  else
+  else if (mode == 1)
     pair_matrix_kernel<1><<<blocks, threads, 0, stream>>>(na, boxes_a, nb, boxes_b, out);
+  else
+    pair_matrix_kernel<2><<<blocks, threads, 0, stream>>>(na, boxes_a, nb, boxes_b, out);
   D3B_LAUNCH_CHECK();
   return D3B_OK;
 }

@@ -68,7 +68,9 @@ def normal_nms_xyxy(bboxes, scores, iou_threshold, post_max_size=None, pixel=Fal
     return _finish(order, keep_idx, keep_count)
 
 
-def boxes_iou_bev(boxes_a, boxes_b, mode=0):
+def boxes_iou_bev(boxes_a, boxes_b, mode=_lib.IOU_BEV_XYXYR):
+    """[na, nb] f32 matrix: mode IOU_BEV_XYXYR / OVERLAP_BEV_XYXYR the iou3d IoU / overlap area of [x1,y1,x2,y2,ry]
+    boxes; mode IOU_BEV_XYWLR the rotate_nms_cc overlap of [cx,cy,w,l,r] boxes that BOX_XYWLR NMS thresholds."""
     a = boxes_a.float().contiguous()
     b = boxes_b.float().contiguous()
     out = torch.zeros((a.shape[0], b.shape[0]), dtype=torch.float32, device=a.device)

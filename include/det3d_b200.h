@@ -368,8 +368,13 @@ int d3b_bev_conv16(const d3b_bev16_params* p, void* stream);
 #define D3B_BOX_XYWLR 1   /* [cx,cy,w,l,r]  : det3d/ops/nms/nms_cpu.py:34-45 + nms_cpu.h:73-169 */
 #define D3B_BOX_XYWLR_RRPN 2 /* [cx,cy,w,l,r]: numba RRPN routine, det3d/ops/nms/nms_gpu.py:180-470 */
 
-/* Pairwise rotated IoU (mode 0) or overlap area (mode 1), out [na, nb].
- * replaces boxes_iou_bev_gpu / boxes_overlap_bev_gpu, det3d/ops/iou3d/src/iou3d.cpp:31-71 */
+/* Pairwise rotated IoU (mode 0) or overlap area (mode 1) of [x1,y1,x2,y2,ry] boxes, out [na, nb].
+ * replaces boxes_iou_bev_gpu / boxes_overlap_bev_gpu, det3d/ops/iou3d/src/iou3d.cpp:31-71
+ * mode 2: the overlap D3B_BOX_XYWLR NMS thresholds, for [cx,cy,w,l,r] boxes (rotate_nms_cc): 0 when the fp32
+ *         IoU of the axis-aligned hulls is <= 0, when the intersection area is not > 0 or the union is not > 0,
+ *         else (float)(inter / union).  The same device function makes the NMS decisions (suppress when
+ *         out >= thresh), so the matrix shows exactly the values the NMS compares.
+ * Any other mode is an invalid argument. */
 int d3b_boxes_iou_bev(const float* boxes_a, int32_t na, const float* boxes_b, int32_t nb,
                       int32_t mode, float* out, void* stream);
 

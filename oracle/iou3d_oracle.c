@@ -184,9 +184,15 @@ static double quad_area(const quad* q) {
   for (int k = 0; k < 4; ++k) { int k1 = (k + 1) & 3; a += (double)q->x[k] * q->y[k1] - (double)q->x[k1] * q->y[k]; }
   return fabs(a) * 0.5;
 }
-static double clip_area(const quad* A, const quad* B) {
-  double px[10], py[10], qx[10], qy[10];
-  int n = 4;
+/* Vertex capacity, as csrc/nms.cu kClipMaxVertices: a clip step keeps k of n vertices and adds one per sign change
+ * (at most 2 min(k, n - k)), so m <= floor(3n / 2) for ANY sign pattern -- rounding can break convexity for
+ * near-duplicate pairs, where exact arithmetic would give at most 8.  4 -> 6 -> 9 -> 13 -> 19. */
+#define CLIP_MAX_VERTICES 19
+
+/* *max_n (when not NULL) receives the largest vertex count of any intermediate polygon */
+static double clip_area_n(const quad* A, const quad* B, int* max_n) {
+  double px[CLIP_MAX_VERTICES], py[CLIP_MAX_VERTICES], qx[CLIP_MAX_VERTICES], qy[CLIP_MAX_VERTICES];
+  int n = 4, top = 4;
   for (int k = 0; k < 4; ++k) { px[k] = A->x[k]; py[k] = A->y[k]; }
   double area2 = 0;
   for (int k = 0; k < 4; ++k) { int k1 = (k + 1) & 3; area2 += (double)B->x[k] * B->y[k1] - (double)B->x[k1] * B->y[k]; }
@@ -205,12 +211,33 @@ static double clip_area(const quad* A, const quad* B) {
       }
     }
     n = m;
+    if (n > top) top = n;
     memcpy(px, qx, sizeof(double) * n); memcpy(py, qy, sizeof(double) * n);
   }
+  if (max_n) *max_n = top;
   if (n < 3) return 0;
   double a = 0;
   for (int k = 0; k < n; ++k) { int k1 = (k + 1 == n) ? 0 : k + 1; a += px[k] * py[k1] - px[k1] * py[k]; }
   return fabs(a) * 0.5;
+}
+static double clip_area(const quad* A, const quad* B) { return clip_area_n(A, B, NULL); }
+
+/* Test access to the clipper.  Corners of one [cx,cy,w,l,r] box as the (B) path builds them: out = x[4], y[4]. */
+void oracle_xywlr_corners(const float* d, float* out) {
+  quad q = make_quad(d);
+  memcpy(out, q.x, sizeof(float) * 4);
+  memcpy(out + 4, q.y, sizeof(float) * 4);
+}
+
+/* Largest intermediate vertex count of clip_area(a[i], b[i]) for n pairs of [cx,cy,w,l,r] boxes -> out[i]. */
+void oracle_clip_max_vertices(const float* da, const float* db, int64_t n, int32_t* out) {
+#pragma omp parallel for schedule(static, 4096)
+  for (int64_t i = 0; i < n; ++i) {
+    quad a = make_quad(da + 5 * i), b = make_quad(db + 5 * i);
+    int top = 0;
+    clip_area_n(&a, &b, &top);
+    out[i] = top;
+  }
 }
 
 /* IoU the (B) path thresholds: 0 when the hulls do not overlap (pair skipped, nms_cpu.h:105). */

@@ -100,6 +100,11 @@ def test_entry_points_validate_before_cuda_without_gpu():
     assert b"format" in L.d3b_last_error()
     assert L.d3b_normal_nms(None, 10, None, 5, 0.5, 10, None, (ctypes.c_int32 * 1)(), None, 0, None) == 1
     assert b"mode" in L.d3b_last_error()
+    # d3b_boxes_iou_bev: modes 0 / 1 (XYXYR IoU / overlap) and 2 (the XYWLR rotate_nms_cc overlap); nothing else
+    assert (_lib.IOU_BEV_XYXYR, _lib.OVERLAP_BEV_XYXYR, _lib.IOU_BEV_XYWLR) == (0, 1, 2)
+    for mode in (3, -1):
+        assert L.d3b_boxes_iou_bev(None, 4, None, 4, mode, None, None) == 1
+        assert b"mode" in L.d3b_last_error()
     one = (ctypes.c_float * 8)()
     st = L.d3b_pillar_features(one, one, one, one, 4, 100, 2, 64, one, one, one, 0.16, 0.16, 0.0, 0.0, one, None)
     assert st == 3 and b"ndim" in L.d3b_last_error()                         # D3B_ERR_UNSUPPORTED
