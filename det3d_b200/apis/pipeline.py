@@ -97,6 +97,13 @@ class InferencePipeline:
         flag = getattr(self.model, "overflow_flag", None)
         return None if flag is None else flag(self.device)
 
+    def set_math(self, math):
+        """Switch the model's convolutions to `math` ("fp16x3", the default; "fp16", single-pass FP16; or "tf32x3") and
+        drop the captured graphs: a graph replays the kernels it was captured with, so one captured under another math
+        would keep running that math."""
+        self.model.set_math(math)
+        self._graphs.clear()
+
     def check_overflow(self, flag_value):
         """Host side of the guard: on a raised flag switch the model to the tf32x3 kernels (permanently: the weights /
         inputs that overflowed once will again) and tell the caller to re-run.  Returns True if a re-run is needed.

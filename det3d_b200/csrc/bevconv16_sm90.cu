@@ -44,12 +44,16 @@ constexpr int kBvTmaWarp = kBvMathWarps;        // first warp of the producer wa
 constexpr int kBvThreads = 32 * (kBvMathWarps + 4);   // 384 (registers are allocated per warpgroup: 168 each)
 constexpr int kBvAStages = 2;
 
-template <int KS, int STRIDE, int COUT>
+// PLANES = 2: FP16x3 (hi and lo planes); 1: single-pass FP16 (hi only).  Every expect-tx byte count below is the sum
+// of the copies it covers: an A stage is 2 halves x PLANES boxes of kPatchBytes (the box make_map encodes: 64 channels x
+// kBvHalfX pixels x kPatchRows rows of f16), a B stage the first PLANES parts of one slot of the packed weight image.
+template <int KS, int STRIDE, int COUT, int PLANES = 2>
 struct BvCfg {
   static constexpr int kPatchRows = STRIDE == 1 ? kBvTileY + KS - 1 : kBvTileY;      // rows in one staged patch
   static constexpr int kPatchBytes = kPatchRows * kBvHalfX * 128;
-  static constexpr int kAStageBytes = 4 * kPatchBytes;                                // {half 0, half 1} x {hi, lo}
-  static constexpr int kBBytes = 2 * COUT * 128;                                      // [B_hi rows | B_lo rows]
+  static constexpr int kAStageBytes = 2 * PLANES * kPatchBytes;                       // {half 0, half 1} x {hi, lo}
+  static constexpr int kSlotHalves = 2 * COUT * kBvKc;                                // packed slot: [W_hi | W_lo]
+  static constexpr int kBBytes = PLANES * COUT * 128;                                 // [B_hi rows | B_lo rows]
   static constexpr int kBStages = COUT >= 128 ? 2 : 4;
   static constexpr int kSmemBytes = kBvAStages * kAStageBytes + kBStages * kBBytes + 1024 + 256;
   // with stride 1 one A stage serves the KS kernel rows of a (kx, kb); with stride > 1 every (ky, kx) has its own
@@ -69,12 +73,13 @@ struct BvGeom {
   int out_channels, out_c0;       // row length of the output tensor and first channel written
 };
 
-template <int KS, int STRIDE, int COUT>
-__global__ void __launch_bounds__(kBvThreads, 1)
-bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, BvGeom g,
-                  const __half* __restrict__ packed, Epi16 epi, __half* __restrict__ out_hi,
-                  __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
-  using Cfg = BvCfg<KS, STRIDE, COUT>;
+// The kernel body for PLANES operand planes; bev_conv16_kernel (FP16x3) and bev_conv16_f16_kernel (single pass) below.
+template <int KS, int STRIDE, int COUT, int PLANES>
+__device__ __forceinline__ void bev_conv16_body(const CUtensorMap* tm_hi, const CUtensorMap* tm_lo, const BvGeom& g,
+                                                const __half* __restrict__ packed, const Epi16& epi,
+                                                __half* __restrict__ out_hi, __half* __restrict__ out_lo,
+                                                float* __restrict__ out_f32, int* __restrict__ overflow) {
+  using Cfg = BvCfg<KS, STRIDE, COUT, PLANES>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_base = smem_base;
@@ -96,8 +101,8 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
     for (int s = 0; s < kBvAStages; ++s) { mbar_init(a_full(s), 1); mbar_init(a_empty(s), kBvMathWarps); }
     for (int s = 0; s < Cfg::kBStages; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), kBvMathWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    tma_prefetch_desc(&tm_hi);
-    tma_prefetch_desc(&tm_lo);
+    tma_prefetch_desc(tm_hi);
+    if constexpr (PLANES == 2) tma_prefetch_desc(tm_lo);
   }
   __syncthreads();
   pdl_wait_prior_grid();             // everything below reads the previous layer's planes or writes buffers it may still read
@@ -119,7 +124,7 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
       for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         int grp, b, y0, x0;
         decode(tile, grp, b, y0, x0);
-        const __half* wgrp = packed + (size_t)grp * k_vol * g.n_kb * (Cfg::kBBytes / 2);
+        const __half* wgrp = packed + (size_t)grp * k_vol * g.n_kb * Cfg::kSlotHalves;
         for (int kb = 0; kb < g.n_kb; ++kb) {
           for (int kx = 0; kx < KS; ++kx) {
             for (int ky0 = 0; ky0 < KS; ky0 += Cfg::kRowsPerAStage) {
@@ -133,8 +138,9 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
 #pragma unroll
               for (int half = 0; half < 2; ++half) {
                 const int cx = (x0 + half * kBvHalfX) * STRIDE + kx - g.pad;
-                tma_load_4d(dst + (2 * half) * Cfg::kPatchBytes, &tm_hi, kb * kBvKc, cx, cy, b, a_full(sa));
-                tma_load_4d(dst + (2 * half + 1) * Cfg::kPatchBytes, &tm_lo, kb * kBvKc, cx, cy, b, a_full(sa));
+                tma_load_4d(dst + (PLANES * half) * Cfg::kPatchBytes, tm_hi, kb * kBvKc, cx, cy, b, a_full(sa));
+                if constexpr (PLANES == 2)
+                  tma_load_4d(dst + (2 * half + 1) * Cfg::kPatchBytes, tm_lo, kb * kBvKc, cx, cy, b, a_full(sa));
               }
               D3B_STAMP(1, a_it);
               ++a_it;
@@ -146,7 +152,7 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
                 D3B_WAIT(b_empty(sb), ((b_it / Cfg::kBStages) & 1u) ^ 1u, 2);
                 mbar_arrive_expect_tx(b_full(sb), Cfg::kBBytes);
                 tma_bulk_g2s(b_base + sb * Cfg::kBBytes,
-                             wgrp + ((size_t)(ky * KS + kx) * g.n_kb + kb) * (Cfg::kBBytes / 2), Cfg::kBBytes, b_full(sb));
+                             wgrp + ((size_t)(ky * KS + kx) * g.n_kb + kb) * Cfg::kSlotHalves, Cfg::kBBytes, b_full(sb));
                 D3B_STAMP(3, b_it);
                 ++b_it;
               }
@@ -183,7 +189,7 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
               const uint32_t b_hi = b_base + sb * Cfg::kBBytes, b_lo = b_hi + COUT * 128;
               // stride 1: kernel row r of the staged patch = the same bytes 8 rows (1024 B) further down
               const uint32_t row_adv = STRIDE == 1 ? (uint32_t)(ky0 + r) * 1024u : 0u;
-              const uint32_t ah = a_base + sa * Cfg::kAStageBytes + (2 * half) * Cfg::kPatchBytes + row_adv;
+              const uint32_t ah = a_base + sa * Cfg::kAStageBytes + (PLANES * half) * Cfg::kPatchBytes + row_adv;
 #pragma unroll
               for (int m = 0; m < 2; ++m) {
                 const uint32_t a_hi = ah + m * 8192u, a_lo = a_hi + Cfg::kPatchBytes;
@@ -197,10 +203,14 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
 #pragma unroll
                   for (int ks = 0; ks < kBvKc / 16; ++ks) {
                     const uint32_t adv = ks * 32;     // 32 bytes along K
-                    // small terms first, the dominant hi.hi product last
-                    wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_lo + adv), gmma_desc_sw128(b_hi + nb + adv), ks > 0 ? 1u : 0u);
-                    wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_lo + nb + adv), 1u);
-                    wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + nb + adv), 1u);
+                    if constexpr (PLANES == 2) {
+                      // small terms first, the dominant hi.hi product last
+                      wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_lo + adv), gmma_desc_sw128(b_hi + nb + adv), ks > 0 ? 1u : 0u);
+                      wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_lo + nb + adv), 1u);
+                      wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + nb + adv), 1u);
+                    } else {
+                      wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + nb + adv), ks > 0 ? 1u : 0u);
+                    }
                   }
                   gmma_commit();
                   gmma_wait();
@@ -245,12 +255,7 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
               v0 = fmaf(v0, sc.x, sh.x); v1 = fmaf(v1, sc.y, sh.y);
             }
             if (epi.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-            if (out_hi) {
-              uint32_t hi, lo;
-              ovf |= split_pack2(v0, v1, hi, lo);
-              *reinterpret_cast<uint32_t*>(out_hi + row_off + col) = hi;
-              *reinterpret_cast<uint32_t*>(out_lo + row_off + col) = lo;
-            }
+            if (out_hi) ovf |= store_pair16<PLANES>(v0, v1, out_hi, out_lo, row_off + col);
             if (out_f32) *reinterpret_cast<float2*>(out_f32 + row_off + col) = make_float2(v0, v1);
           }
         }
@@ -259,6 +264,23 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
     if (ovf && overflow) atomicOr(overflow, 1);
   }
   D3B_CTA_MARK(1, epi.seq);
+}
+
+template <int KS, int STRIDE, int COUT>
+__global__ void __launch_bounds__(kBvThreads, 1)
+bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, BvGeom g,
+                  const __half* __restrict__ packed, Epi16 epi, __half* __restrict__ out_hi,
+                  __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
+  bev_conv16_body<KS, STRIDE, COUT, 2>(&tm_hi, &tm_lo, g, packed, epi, out_hi, out_lo, out_f32, overflow);
+}
+
+// Single-pass FP16: one A box per half and W_hi only per stage, one wgmma(A_hi, W_hi) per k-step (tm_lo, out_lo unused).
+template <int KS, int STRIDE, int COUT>
+__global__ void __launch_bounds__(kBvThreads, 1)
+bev_conv16_f16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, BvGeom g,
+                      const __half* __restrict__ packed, Epi16 epi, __half* __restrict__ out_hi,
+                      __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
+  bev_conv16_body<KS, STRIDE, COUT, 1>(&tm_hi, &tm_lo, g, packed, epi, out_hi, out_lo, out_f32, overflow);
 }
 
 // ======================================================================================================================
@@ -273,19 +295,26 @@ bev_conv16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_consta
 // the pixel-stationary kernel: bit-identical to it.
 //  * A stage = one box per plane, 64 channels x 8 pixels x 18 rows (18 KB); block m reads kernel row ky at
 //    m * 8192 + ky * 1024.  B stage = [W_hi | W_lo] of one (kb, kx, ky).  Three stages of each.
+//  * Single-pass FP16 (PLANES = 1): the hi box and W_hi alone per stage, one MMA per k-step (4 per slot).
 constexpr int kPlCout = 128;
 constexpr int kPlStages = 3;
 constexpr int kPlPatchBytes = (kBvTileY + 2) * kBvHalfX * 128;    // 18432
-constexpr int kPlAStageBytes = 2 * kPlPatchBytes;                 // hi, lo
-constexpr int kPlBBytes = 2 * kPlCout * 128;                      // [W_hi rows | W_lo rows]
-constexpr int kPlSmemBytes = kPlStages * (kPlAStageBytes + kPlBBytes) + 1024 + 256;
+constexpr int kPlSlotHalves = 2 * kPlCout * kBvKc;                // packed slot: [W_hi | W_lo]
+template <int PLANES>
+struct PlCfg {
+  static constexpr int kAStageBytes = PLANES * kPlPatchBytes;     // hi, lo: PLANES boxes of kPlPatchBytes
+  static constexpr int kBBytes = PLANES * kPlCout * 128;          // [W_hi rows | W_lo rows]
+  static constexpr int kSmemBytes = kPlStages * (kAStageBytes + kBBytes) + 1024 + 256;
+};
 constexpr int kPlConsumerRegs = 232, kPlProducerRegs = 40;        // 2 * 232 + 40 <= 512 per thread triple
 static_assert(2 * kPlConsumerRegs + kPlProducerRegs <= 512, "register budget of one SM");
 
-__global__ void __launch_bounds__(kBvThreads, 1)
-bev_conv16_pl_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, BvGeom g,
-                     const __half* __restrict__ packed, Epi16 epi, __half* __restrict__ out_hi,
-                     __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
+template <int PLANES>
+__device__ __forceinline__ void bev_conv16_pl_body(const CUtensorMap* tm_hi, const CUtensorMap* tm_lo, const BvGeom& g,
+                                                   const __half* __restrict__ packed, const Epi16& epi,
+                                                   __half* __restrict__ out_hi, __half* __restrict__ out_lo,
+                                                   float* __restrict__ out_f32, int* __restrict__ overflow) {
+  constexpr int kPlAStageBytes = PlCfg<PLANES>::kAStageBytes, kPlBBytes = PlCfg<PLANES>::kBBytes;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_base = smem_base;
@@ -309,8 +338,8 @@ bev_conv16_pl_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
       mbar_init(b_full(s), 1); mbar_init(b_empty(s), kBvMathWarps);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    tma_prefetch_desc(&tm_hi);
-    tma_prefetch_desc(&tm_lo);
+    tma_prefetch_desc(tm_hi);
+    if constexpr (PLANES == 2) tma_prefetch_desc(tm_lo);
   }
   __syncthreads();
   pdl_wait_prior_grid();             // everything below reads the previous layer's planes or writes buffers it may still read
@@ -332,20 +361,21 @@ bev_conv16_pl_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
       for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         int grp, b, y0, x0;
         decode(tile, grp, b, y0, x0);
-        const __half* wgrp = packed + (size_t)grp * 9 * g.n_kb * (kPlBBytes / 2);
+        const __half* wgrp = packed + (size_t)grp * 9 * g.n_kb * kPlSlotHalves;
         for (int kb = 0; kb < g.n_kb; ++kb) {
           for (int kx = 0; kx < 3; ++kx, ++a_it) {
             const uint32_t sa = a_it % kPlStages;
             D3B_WAIT(a_empty(sa), ((a_it / kPlStages) & 1u) ^ 1u, 1);
             mbar_arrive_expect_tx(a_full(sa), kPlAStageBytes);
             const uint32_t dst = a_base + sa * kPlAStageBytes;
-            tma_load_4d(dst, &tm_hi, kb * kBvKc, x0 + kx - g.pad, y0 - g.pad, b, a_full(sa));
-            tma_load_4d(dst + kPlPatchBytes, &tm_lo, kb * kBvKc, x0 + kx - g.pad, y0 - g.pad, b, a_full(sa));
+            tma_load_4d(dst, tm_hi, kb * kBvKc, x0 + kx - g.pad, y0 - g.pad, b, a_full(sa));
+            if constexpr (PLANES == 2)
+              tma_load_4d(dst + kPlPatchBytes, tm_lo, kb * kBvKc, x0 + kx - g.pad, y0 - g.pad, b, a_full(sa));
             for (int ky = 0; ky < 3; ++ky, ++b_it) {
               const uint32_t sb = b_it % kPlStages;
               D3B_WAIT(b_empty(sb), ((b_it / kPlStages) & 1u) ^ 1u, 2);
               mbar_arrive_expect_tx(b_full(sb), kPlBBytes);
-              tma_bulk_g2s(b_base + sb * kPlBBytes, wgrp + ((size_t)(ky * 3 + kx) * g.n_kb + kb) * (kPlBBytes / 2),
+              tma_bulk_g2s(b_base + sb * kPlBBytes, wgrp + ((size_t)(ky * 3 + kx) * g.n_kb + kb) * kPlSlotHalves,
                            kPlBBytes, b_full(sb));
             }
           }
@@ -377,10 +407,14 @@ bev_conv16_pl_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
 #pragma unroll
         for (int ks = 0; ks < kBvKc / 16; ++ks) {
           const uint32_t adv = ks * 32;
-          // small terms first, the dominant hi.hi product last (the order of the pixel-stationary kernel)
-          wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_lo + adv), gmma_desc_sw128(b_hi + adv), ks > 0 ? 1u : 0u);
-          wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_lo + adv), 1u);
-          wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + adv), 1u);
+          if constexpr (PLANES == 2) {
+            // small terms first, the dominant hi.hi product last (the order of the pixel-stationary kernel)
+            wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_lo + adv), gmma_desc_sw128(b_hi + adv), ks > 0 ? 1u : 0u);
+            wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_lo + adv), 1u);
+            wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + adv), 1u);
+          } else {
+            wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + adv), ks > 0 ? 1u : 0u);
+          }
         }
         gmma_commit();
       };
@@ -444,12 +478,13 @@ bev_conv16_pl_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
           if (epi.bias) { v0 += bb.x; v1 += bb.y; }
           if (epi.scale) { v0 = fmaf(v0, sc.x, sh.x); v1 = fmaf(v1, sc.y, sh.y); }
           if (epi.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-          if (out_hi) {
+          if (out_hi && PLANES == 2) {
             uint32_t hi, lo;
             ovf |= split_pack2(v0, v1, hi, lo);
             *reinterpret_cast<uint32_t*>(out_hi + row_off[h] + col) = hi;
             *reinterpret_cast<uint32_t*>(out_lo + row_off[h] + col) = lo;
           }
+          if (out_hi && PLANES == 1) ovf |= store_pair16<1>(v0, v1, out_hi, out_lo, row_off[h] + col);
           if (out_f32) *reinterpret_cast<float2*>(out_f32 + row_off[h] + col) = make_float2(v0, v1);
         }
       }
@@ -459,6 +494,21 @@ bev_conv16_pl_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
     }
   }
   D3B_CTA_MARK(1, epi.seq);
+}
+
+__global__ void __launch_bounds__(kBvThreads, 1)
+bev_conv16_pl_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, BvGeom g,
+                     const __half* __restrict__ packed, Epi16 epi, __half* __restrict__ out_hi,
+                     __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
+  bev_conv16_pl_body<2>(&tm_hi, &tm_lo, g, packed, epi, out_hi, out_lo, out_f32, overflow);
+}
+
+// Single-pass FP16 (tm_lo, out_lo unused).
+__global__ void __launch_bounds__(kBvThreads, 1)
+bev_conv16_pl_f16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, BvGeom g,
+                         const __half* __restrict__ packed, Epi16 epi, __half* __restrict__ out_hi,
+                         __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
+  bev_conv16_pl_body<1>(&tm_hi, &tm_lo, g, packed, epi, out_hi, out_lo, out_f32, overflow);
 }
 
 // ---- host side: tensor maps through the driver entry point (libcuda is not linked: CPU hosts must dlopen us) ----------
@@ -503,16 +553,19 @@ static int make_map(CUtensorMap* map, const void* base, int batch, int h, int w,
 }
 
 // What both kernels are launched with: the tensor maps of the input planes (boxes of box_w pixels x box_h rows) and the
-// epilogue parameters.
-static int bev_args(const d3b_bev16_params* p, int box_w, int box_h, int stride, CUtensorMap* tm_hi, CUtensorMap* tm_lo,
-                    Epi16* e) {
+// epilogue parameters.  Single pass (planes = 1): no lo plane; tm_lo repeats tm_hi and is never read.
+static int bev_args(const d3b_bev16_params* p, int planes, int box_w, int box_h, int stride, CUtensorMap* tm_hi,
+                    CUtensorMap* tm_lo, Epi16* e) {
   int st = make_map(tm_hi, p->in_hi, p->batch, p->h_in, p->w_in, p->c_in, box_w, box_h, stride);
-  if (st == D3B_OK) st = make_map(tm_lo, p->in_lo, p->batch, p->h_in, p->w_in, p->c_in, box_w, box_h, stride);
+  if (st == D3B_OK) {
+    if (planes == 2) st = make_map(tm_lo, p->in_lo, p->batch, p->h_in, p->w_in, p->c_in, box_w, box_h, stride);
+    else *tm_lo = *tm_hi;
+  }
   if (st != D3B_OK) return st;
   e->bias = p->bias; e->scale = p->scale; e->shift = p->shift;
   e->res_hi = nullptr; e->res_lo = nullptr;
   e->acc_scale = p->acc_scale; e->relu = p->relu;
-  e->corr = trunc_correction(p->c_in);
+  e->corr = trunc_correction(p->c_in, planes == 2 ? 3 : 1);
   static std::atomic<int> launch_seq{0};
   e->seq = launch_seq.fetch_add(1, std::memory_order_relaxed);
   return D3B_OK;
@@ -524,16 +577,17 @@ static int bev_grid(const BvGeom& g) {
   return n_tiles < kNumSMs ? n_tiles : kNumSMs;
 }
 
-template <int KS, int STRIDE, int COUT>
+template <int KS, int STRIDE, int COUT, int PLANES>
 static int launch_bev(const d3b_bev16_params* p, const BvGeom& g, cudaStream_t stream) {
-  using Cfg = BvCfg<KS, STRIDE, COUT>;
+  using Cfg = BvCfg<KS, STRIDE, COUT, PLANES>;
+  constexpr auto kernel = PLANES == 2 ? bev_conv16_kernel<KS, STRIDE, COUT> : bev_conv16_f16_kernel<KS, STRIDE, COUT>;
   static SmemOptIn optin;
-  D3B_CUDA(ensure_dynamic_smem(bev_conv16_kernel<KS, STRIDE, COUT>, Cfg::kSmemBytes, optin));
+  D3B_CUDA(ensure_dynamic_smem(kernel, Cfg::kSmemBytes, optin));
   CUtensorMap tm_hi, tm_lo;
   Epi16 e;
-  const int st = bev_args(p, kBvHalfX, Cfg::kPatchRows, STRIDE, &tm_hi, &tm_lo, &e);
+  const int st = bev_args(p, PLANES, kBvHalfX, Cfg::kPatchRows, STRIDE, &tm_hi, &tm_lo, &e);
   if (st != D3B_OK) return st;
-  D3B_CUDA(launch_maybe_pdl(bev_conv16_kernel<KS, STRIDE, COUT>, dim3(bev_grid(g)), dim3(kBvThreads), Cfg::kSmemBytes,
+  D3B_CUDA(launch_maybe_pdl(kernel, dim3(bev_grid(g)), dim3(kBvThreads), Cfg::kSmemBytes,
                             stream, tm_hi, tm_lo, g, (const __half*)p->weight_packed, e, (__half*)p->out_hi,
                             (__half*)p->out_lo, p->out_f32, (int*)p->overflow));
   D3B_LAUNCH_CHECK();
@@ -541,15 +595,17 @@ static int launch_bev(const d3b_bev16_params* p, const BvGeom& g, cudaStream_t s
 }
 
 // pipelined variant: 3x3, stride 1, output blocks of 128 channels, C_in % 64 == 0, no sub-pixel groups
+template <int PLANES>
 static int launch_bev_pl(const d3b_bev16_params* p, BvGeom g, cudaStream_t stream) {
+  constexpr auto kernel = PLANES == 2 ? bev_conv16_pl_kernel : bev_conv16_pl_f16_kernel;
   static SmemOptIn optin;
-  D3B_CUDA(ensure_dynamic_smem(bev_conv16_pl_kernel, kPlSmemBytes, optin));
+  D3B_CUDA(ensure_dynamic_smem(kernel, PlCfg<PLANES>::kSmemBytes, optin));
   CUtensorMap tm_hi, tm_lo;
   Epi16 e;
-  const int st = bev_args(p, kBvHalfX, kBvTileY + 2, 1, &tm_hi, &tm_lo, &e);
+  const int st = bev_args(p, PLANES, kBvHalfX, kBvTileY + 2, 1, &tm_hi, &tm_lo, &e);
   if (st != D3B_OK) return st;
   g.tiles_x = div_up(g.w_out, kBvHalfX);     // tiles of 16 rows x 8 columns
-  D3B_CUDA(launch_maybe_pdl(bev_conv16_pl_kernel, dim3(bev_grid(g)), dim3(kBvThreads), kPlSmemBytes, stream, tm_hi, tm_lo,
+  D3B_CUDA(launch_maybe_pdl(kernel, dim3(bev_grid(g)), dim3(kBvThreads), PlCfg<PLANES>::kSmemBytes, stream, tm_hi, tm_lo,
                             g, (const __half*)p->weight_packed, e, (__half*)p->out_hi, (__half*)p->out_lo, p->out_f32,
                             (int*)p->overflow));
   D3B_LAUNCH_CHECK();
@@ -562,7 +618,14 @@ using namespace d3b;
 
 extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  D3B_REQUIRE(p && p->in_hi && p->in_lo && p->weight_packed, "d3b_bev_conv16: null argument");
+  D3B_REQUIRE(p && p->in_hi && p->weight_packed, "d3b_bev_conv16: null argument");
+  PlanePairs pp;
+  pp.add(p->in_hi, p->in_lo);
+  pp.add(p->out_hi, p->out_lo);
+  D3B_REQUIRE(pp.consistent(),
+              "d3b_bev_conv16: give in_lo and out_lo with their hi planes (FP16x3) or neither (single-pass FP16); got "
+              "in_lo %s, out_lo %s", p->in_lo ? "set" : "NULL", p->out_lo ? "set" : "NULL");
+  const bool two = pp.planes() == 2;
   D3B_REQUIRE(p->batch >= 1 && p->h_in >= 1 && p->w_in >= 1 && p->c_in >= 16 && p->c_in % 16 == 0,
               "d3b_bev_conv16: bad input shape [%d,%d,%d,%d] (C_in must be a multiple of 16)", p->batch, p->h_in, p->w_in, p->c_in);
   // kernel = stride = s (2..4): the strided Conv2d deblock; it tiles the input exactly, so it takes no padding
@@ -574,8 +637,7 @@ extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
               "d3b_bev_conv16: pad %d not built for ksize %d stride %d", p->pad, p->ksize, p->stride);
   D3B_REQUIRE(p->up >= 1 && p->up <= 4 && p->cgroups >= 1 && p->groups == p->cgroups * p->up * p->up,
               "d3b_bev_conv16: groups %d != cgroups %d * up^2 (up %d)", p->groups, p->cgroups, p->up);
-  D3B_REQUIRE((p->out_hi != nullptr) == (p->out_lo != nullptr) && (p->out_hi || p->out_f32),
-              "d3b_bev_conv16: give out_hi + out_lo and/or out_f32");
+  D3B_REQUIRE(p->out_hi || p->out_f32, "d3b_bev_conv16: give out_hi (+ out_lo) and/or out_f32");
   D3B_REQUIRE((p->scale == nullptr) == (p->shift == nullptr), "d3b_bev_conv16: scale and shift go together");
   D3B_REQUIRE(p->out_channels % 8 == 0 && p->out_c0 % 8 == 0 && p->out_c0 + p->cgroups * p->c_out <= p->out_channels,
               "d3b_bev_conv16: output channel slice [%d, %d) does not fit rows of %d", p->out_c0,
@@ -600,15 +662,15 @@ extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
   // pixel-stationary kernel for every other shape.  Variant 0 (pixel-stationary everywhere) is the reference the
   // pipelined kernel reproduces bit for bit.
   const bool s1_blocks = p->ksize == 3 && p->stride == 1 && p->c_out == kPlCout && p->c_in % kBvKc == 0 && p->up == 1;
-  if (bev_variant() == 2 && s1_blocks) return launch_bev_pl(p, g, stream);
-#define D3B_BEV_CASE(KS, ST)                                                   \
-  if (p->ksize == KS && p->stride == ST) {                                     \
-    switch (p->c_out) {                                                        \
-      case 32: return launch_bev<KS, ST, 32>(p, g, stream);                    \
-      case 64: return launch_bev<KS, ST, 64>(p, g, stream);                    \
-      case 128: return launch_bev<KS, ST, 128>(p, g, stream);                  \
-      default: break;                                                          \
-    }                                                                          \
+  if (bev_variant() == 2 && s1_blocks) return two ? launch_bev_pl<2>(p, g, stream) : launch_bev_pl<1>(p, g, stream);
+#define D3B_BEV_CASE(KS, ST)                                                                                        \
+  if (p->ksize == KS && p->stride == ST) {                                                                          \
+    switch (p->c_out) {                                                                                             \
+      case 32: return two ? launch_bev<KS, ST, 32, 2>(p, g, stream) : launch_bev<KS, ST, 32, 1>(p, g, stream);       \
+      case 64: return two ? launch_bev<KS, ST, 64, 2>(p, g, stream) : launch_bev<KS, ST, 64, 1>(p, g, stream);       \
+      case 128: return two ? launch_bev<KS, ST, 128, 2>(p, g, stream) : launch_bev<KS, ST, 128, 1>(p, g, stream);    \
+      default: break;                                                                                               \
+    }                                                                                                               \
   }
   D3B_BEV_CASE(3, 1)
   D3B_BEV_CASE(3, 2)

@@ -283,10 +283,11 @@ constexpr float kTruncLossPerMma = 1.4901161e-8f;   // 2^-26
 // partials to the running sums with round-to-nearest; the epilogue then scales the sum by 1 + c, computed as
 // fmaf(v, c, v) (1 + 12 * 2^-26 is not an fp32 number: a factor would round to 1 + 16 * 2^-26).  c is the layer's mean
 // n * kTruncLossPerMma: 12 * 2^-26 when C_in (per slot) is a multiple of 64; a ragged last slice chains fewer MMAs and
-// is weighted by its channels.
-__host__ __device__ inline float trunc_correction(int c_slot) {
+// is weighted by its channels.  The single-pass FP16 kernels issue one MMA per k-step (mmas_per_kstep = 1): n = n_ks,
+// 4 * 2^-26 for a full slice.
+__host__ __device__ inline float trunc_correction(int c_slot, int mmas_per_kstep = 3) {
   const int full = c_slot / 64, rest = c_slot - 64 * full;
-  const float n = (float)(12 * 64 * full + 3 * ((rest + 15) / 16) * rest) / (float)c_slot;
+  const float n = (float)(4 * mmas_per_kstep * 64 * full + mmas_per_kstep * ((rest + 15) / 16) * rest) / (float)c_slot;
   return n * kTruncLossPerMma;
 }
 

@@ -43,10 +43,13 @@ constexpr int kOsTileM = 128;
 constexpr int kOsKc = 64;                                  // channels per stage = one 128-byte swizzle row of f16
 constexpr int kOsABytes = kOsTileM * 128;                  // one A plane tile (hi or lo)
 
-template <int COUT>
+// PLANES = 2: FP16x3 (hi and lo of activations and weights); 1: single-pass FP16 (hi only).  A B stage holds the first
+// PLANES parts of one slot of the packed weight image, whose slot stride is kSlotHalves in both modes.
+template <int COUT, int PLANES = 2>
 struct OsCfg {
-  static constexpr int kBBytes = 2 * COUT * 128;           // [B_hi rows | B_lo rows]
-  static constexpr int kStageBytes = 2 * kOsABytes + kBBytes;
+  static constexpr int kSlotHalves = 2 * COUT * kOsKc;     // packed[slot][kb] = [W_hi rows | W_lo rows]
+  static constexpr int kBBytes = PLANES * COUT * 128;      // [B_hi rows | B_lo rows], or B_hi rows
+  static constexpr int kStageBytes = PLANES * kOsABytes + kBBytes;
   static constexpr int kStages = COUT >= 128 ? 3 : 4;
   // One gather group per pipeline stage: group g only ever fills stage g.  (A group waits for "stage free" on the
   // PARITY of the stage's empty barrier; that is unambiguous only if the group itself has seen the previous use of
@@ -66,6 +69,7 @@ struct OsCfg {
 
 // Fused epilogue on 16 consecutive output channels of one row (the FFMA first layer: its sums are not truncated, so no
 // correction); returns true if a value left the f16 range.
+template <int PLANES>
 __device__ __forceinline__ bool epilogue16(float (&v)[16], const Epi16& e, size_t row_off, int col, __half* out_hi,
                                            __half* out_lo, float* out_f32) {
 #pragma unroll
@@ -89,15 +93,26 @@ __device__ __forceinline__ bool epilogue16(float (&v)[16], const Epi16& e, size_
   if (e.res_hi) {
 #pragma unroll
     for (int q = 0; q < 16; q += 8) {
-      const uint4 h = __ldg(reinterpret_cast<const uint4*>(e.res_hi + row_off + col + q));
-      const uint4 l = __ldg(reinterpret_cast<const uint4*>(e.res_lo + row_off + col + q));
-      const uint32_t hw[4] = {h.x, h.y, h.z, h.w}, lw[4] = {l.x, l.y, l.z, l.w};
+      if constexpr (PLANES == 2) {
+        const uint4 h = __ldg(reinterpret_cast<const uint4*>(e.res_hi + row_off + col + q));
+        const uint4 l = __ldg(reinterpret_cast<const uint4*>(e.res_lo + row_off + col + q));
+        const uint32_t hw[4] = {h.x, h.y, h.z, h.w}, lw[4] = {l.x, l.y, l.z, l.w};
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&hw[j]));
-        const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&lw[j]));
-        v[q + 2 * j] += fh.x + fl.x;          // hi + lo is exact in fp32 (22 bits)
-        v[q + 2 * j + 1] += fh.y + fl.y;
+        for (int j = 0; j < 4; ++j) {
+          const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&hw[j]));
+          const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&lw[j]));
+          v[q + 2 * j] += fh.x + fl.x;          // hi + lo is exact in fp32 (22 bits)
+          v[q + 2 * j + 1] += fh.y + fl.y;
+        }
+      } else {
+        const uint4 h = __ldg(reinterpret_cast<const uint4*>(e.res_hi + row_off + col + q));
+        const uint32_t hw[4] = {h.x, h.y, h.z, h.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&hw[j]));
+          v[q + 2 * j] += fh.x;
+          v[q + 2 * j + 1] += fh.y;
+        }
       }
     }
   }
@@ -106,7 +121,7 @@ __device__ __forceinline__ bool epilogue16(float (&v)[16], const Epi16& e, size_
 #pragma unroll
     for (int q = 0; q < 16; ++q) v[q] = fmaxf(v[q], 0.f);
   }
-  if (out_hi) {
+  if (out_hi && PLANES == 2) {
     uint32_t hi[8], lo[8];
 #pragma unroll
     for (int q = 0; q < 16; q += 2) ovf |= split_pack2(v[q], v[q + 1], hi[q >> 1], lo[q >> 1]);
@@ -117,6 +132,17 @@ __device__ __forceinline__ bool epilogue16(float (&v)[16], const Epi16& e, size_
     pl[0] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
     pl[1] = make_uint4(lo[4], lo[5], lo[6], lo[7]);
   }
+  if (out_hi && PLANES == 1) {
+    uint32_t hi[8];
+#pragma unroll
+    for (int q = 0; q < 16; q += 2) {
+      hi[q >> 1] = pack_half2(__float2half_rn(v[q]), __float2half_rn(v[q + 1]));
+      ovf |= f16_out_of_range(v[q]) | f16_out_of_range(v[q + 1]);
+    }
+    uint4* ph = reinterpret_cast<uint4*>(out_hi + row_off + col);
+    ph[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    ph[1] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
+  }
   if (out_f32) {
     float4* pf = reinterpret_cast<float4*>(out_f32 + row_off + col);
 #pragma unroll
@@ -126,6 +152,7 @@ __device__ __forceinline__ bool epilogue16(float (&v)[16], const Epi16& e, size_
 }
 
 // The same epilogue on the two consecutive output channels a wgmma accumulator fragment holds, with the correction.
+template <int PLANES>
 __device__ __forceinline__ bool epilogue2(float v0, float v1, const Epi16& e, size_t row_off, int col, __half* out_hi,
                                           __half* out_lo, float* out_f32) {
   v0 *= e.acc_scale;
@@ -142,19 +169,13 @@ __device__ __forceinline__ bool epilogue2(float v0, float v1, const Epi16& e, si
     v0 = fmaf(v0, s.x, t.x); v1 = fmaf(v1, s.y, t.y);
   }
   if (e.res_hi) {
-    const float2 fh = __half22float2(__ldg(reinterpret_cast<const __half2*>(e.res_hi + row_off + col)));
-    const float2 fl = __half22float2(__ldg(reinterpret_cast<const __half2*>(e.res_lo + row_off + col)));
-    v0 += fh.x + fl.x;          // hi + lo is exact in fp32 (22 bits)
-    v1 += fh.y + fl.y;
+    const float2 r = load_pair16<PLANES>(e.res_hi, e.res_lo, row_off + col);
+    v0 += r.x;
+    v1 += r.y;
   }
   if (e.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
   bool ovf = false;
-  if (out_hi) {
-    uint32_t hi, lo;
-    ovf = split_pack2(v0, v1, hi, lo);
-    *reinterpret_cast<uint32_t*>(out_hi + row_off + col) = hi;
-    *reinterpret_cast<uint32_t*>(out_lo + row_off + col) = lo;
-  }
+  if (out_hi) ovf = store_pair16<PLANES>(v0, v1, out_hi, out_lo, row_off + col);
   if (out_f32) *reinterpret_cast<float2*>(out_f32 + row_off + col) = make_float2(v0, v1);
   return ovf;
 }
@@ -175,13 +196,14 @@ __device__ __forceinline__ unsigned int os16_slot_mask(unsigned int offset_mask,
   return r;
 }
 
-template <int COUT>
-__global__ void __launch_bounds__(OsCfg<COUT>::kThreads, 1)
-spconv_os16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ in_lo, const int* __restrict__ nbr,
-                   const unsigned int* __restrict__ tile_mask, const int* __restrict__ n_out_p, int out_cap, int c_in,
-                   int n_kb, int pack, int k_vol, const __half* __restrict__ packed, Epi16 epi, __half* __restrict__ out_hi,
-                   __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
-  using Cfg = OsCfg<COUT>;
+// The kernel body for PLANES operand planes; spconv_os16_kernel (FP16x3) and spconv_os16_f16_kernel (single pass) below.
+template <int COUT, int PLANES>
+__device__ __forceinline__ void spconv_os16_body(
+    const __half* __restrict__ in_hi, const __half* __restrict__ in_lo, const int* __restrict__ nbr,
+    const unsigned int* __restrict__ tile_mask, const int* __restrict__ n_out_p, int out_cap, int c_in, int n_kb, int pack,
+    int k_vol, const __half* __restrict__ packed, const Epi16& epi, __half* __restrict__ out_hi, __half* __restrict__ out_lo,
+    float* __restrict__ out_f32, int* __restrict__ overflow) {
+  using Cfg = OsCfg<COUT, PLANES>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -231,8 +253,8 @@ spconv_os16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ 
         if (warp == 0 && lane == 0) D3B_STAMP(6, it);
         D3B_WAIT(full_bar(s), ph, 3);
         const uint32_t a_hi = smem_base + s * Cfg::kStageBytes + wg * 8192u;   // rows 64 wg .. 64 wg + 63
-        const uint32_t a_lo = a_hi + kOsABytes;
-        const uint32_t b_hi = smem_base + s * Cfg::kStageBytes + 2 * kOsABytes;
+        const uint32_t a_lo = a_hi + kOsABytes;                                  // (PLANES = 2 only)
+        const uint32_t b_hi = smem_base + s * Cfg::kStageBytes + PLANES * kOsABytes;
         const uint32_t b_lo = b_hi + COUT * 128;
 #pragma unroll
         for (int np = 0; np < COUT / Cfg::kPassN; ++np) {
@@ -244,10 +266,14 @@ spconv_os16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ 
 #pragma unroll
           for (int ks = 0; ks < kOsKc / 16; ++ks) {
             const uint32_t adv = ks * 32;               // 16 f16 = 32 bytes along K
-            // small terms first, the dominant hi.hi product last
-            wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_lo + adv), gmma_desc_sw128(b_hi + nb + adv), ks > 0 ? 1u : 0u);
-            wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_lo + nb + adv), 1u);
-            wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + nb + adv), 1u);
+            if constexpr (PLANES == 2) {
+              // small terms first, the dominant hi.hi product last
+              wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_lo + adv), gmma_desc_sw128(b_hi + nb + adv), ks > 0 ? 1u : 0u);
+              wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_lo + nb + adv), 1u);
+              wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + nb + adv), 1u);
+            } else {
+              wgmma_f16<Cfg::kPassN>(part, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + nb + adv), ks > 0 ? 1u : 0u);
+            }
           }
           gmma_commit();
           gmma_wait();
@@ -265,7 +291,7 @@ spconv_os16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ 
         if (o >= n_out) continue;
 #pragma unroll
         for (int jn = 0; jn < COUT / 8; ++jn)
-          ovf |= epilogue2(acc[4 * jn + 2 * h], acc[4 * jn + 2 * h + 1], epi, (size_t)o * COUT, jn * 8 + 2 * (lane & 3),
+          ovf |= epilogue2<PLANES>(acc[4 * jn + 2 * h], acc[4 * jn + 2 * h + 1], epi, (size_t)o * COUT, jn * 8 + 2 * (lane & 3),
                            out_hi, out_lo, out_f32);
       }
     }
@@ -336,7 +362,7 @@ spconv_os16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ 
         const uint32_t stage = smem_base + s * Cfg::kStageBytes;
         if (issues_tma) {
           mbar_arrive_expect_tx(full_bar(s), Cfg::kBBytes);
-          tma_bulk_g2s(stage + 2 * kOsABytes, packed + ((size_t)koff_s[n] * n_kb + kb) * (Cfg::kBBytes / 2), Cfg::kBBytes,
+          tma_bulk_g2s(stage + PLANES * kOsABytes, packed + ((size_t)koff_s[n] * n_kb + kb) * Cfg::kSlotHalves, Cfg::kBBytes,
                        full_bar(s));
         }
         {   // chunks past C_in are zero-filled (the consumers always multiply the full 64-channel slot)
@@ -355,7 +381,7 @@ spconv_os16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ 
               const size_t off = live ? (size_t)srcs[u] * c_in + ch : 0;
               const uint32_t dst = stage + sw128_offset(row, c);
               cp_async16(dst, in_hi + off, live ? 16u : 0u);
-              cp_async16(dst + kOsABytes, in_lo + off, live ? 16u : 0u);
+              if constexpr (PLANES == 2) cp_async16(dst + kOsABytes, in_lo + off, live ? 16u : 0u);
             }
           }
         }
@@ -371,16 +397,37 @@ spconv_os16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ 
   D3B_CTA_MARK(1, epi.seq);
 }
 
+template <int COUT>
+__global__ void __launch_bounds__(OsCfg<COUT>::kThreads, 1)
+spconv_os16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ in_lo, const int* __restrict__ nbr,
+                   const unsigned int* __restrict__ tile_mask, const int* __restrict__ n_out_p, int out_cap, int c_in,
+                   int n_kb, int pack, int k_vol, const __half* __restrict__ packed, Epi16 epi, __half* __restrict__ out_hi,
+                   __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
+  spconv_os16_body<COUT, 2>(in_hi, in_lo, nbr, tile_mask, n_out_p, out_cap, c_in, n_kb, pack, k_vol, packed, epi, out_hi,
+                            out_lo, out_f32, overflow);
+}
+
+// Single-pass FP16: the same kernel on the hi planes alone, one wgmma(A_hi, W_hi) per k-step (in_lo / out_lo unused).
+template <int COUT>
+__global__ void __launch_bounds__(OsCfg<COUT, 1>::kThreads, 1)
+spconv_os16_f16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ in_lo, const int* __restrict__ nbr,
+                       const unsigned int* __restrict__ tile_mask, const int* __restrict__ n_out_p, int out_cap, int c_in,
+                       int n_kb, int pack, int k_vol, const __half* __restrict__ packed, Epi16 epi,
+                       __half* __restrict__ out_hi, __half* __restrict__ out_lo, float* __restrict__ out_f32,
+                       int* __restrict__ overflow) {
+  spconv_os16_body<COUT, 1>(in_hi, in_lo, nbr, tile_mask, n_out_p, out_cap, c_in, n_kb, pack, k_vol, packed, epi, out_hi,
+                            out_lo, out_f32, overflow);
+}
+
 // ---- first layer: fp32 rows with a handful of channels (C_in <= 16: the voxel mean, 4 or 5 features) -----------------
 // 2*27*C_in*C_out flops per row -- nothing for the tensor cores.  fp32 FFMA, output-stationary, same epilogue and
 // output format as the tensor-core kernel.  Four lanes share a (row, 16-column part), each taking every fourth offset (their
 // neighbour-index loads are independent and in flight together: the kernel is pure latency), combined by a fixed shuffle tree.
-template <int COUT>
-__global__ void __launch_bounds__(256)
-spconv_first16_kernel(const float* __restrict__ feat_in, const int* __restrict__ nbr, const int* __restrict__ n_out_p,
-                      int out_cap, int c_in, int in_ld, int k_vol, const float* __restrict__ weight, Epi16 epi,
-                      __half* __restrict__ out_hi, __half* __restrict__ out_lo, float* __restrict__ out_f32,
-                      int* __restrict__ overflow) {
+template <int COUT, int PLANES>
+__device__ __forceinline__ void spconv_first16_body(
+    const float* __restrict__ feat_in, const int* __restrict__ nbr, const int* __restrict__ n_out_p, int out_cap, int c_in,
+    int in_ld, int k_vol, const float* __restrict__ weight, Epi16 epi, __half* __restrict__ out_hi,
+    __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
   extern __shared__ float w_s[];                 // [k_vol][c_in][COUT]
   for (int i = threadIdx.x; i < k_vol * c_in * COUT; i += blockDim.x) w_s[i] = weight[i];
   __syncthreads();
@@ -421,9 +468,30 @@ spconv_first16_kernel(const float* __restrict__ feat_in, const int* __restrict__
       acc[q] += __shfl_xor_sync(0xffffffffu, acc[q], 1);
       acc[q] += __shfl_xor_sync(0xffffffffu, acc[q], 2);
     }
-    if (on && sub == 0) ovf |= epilogue16(acc, epi, (size_t)o * COUT, col, out_hi, out_lo, out_f32);
+    if (on && sub == 0) ovf |= epilogue16<PLANES>(acc, epi, (size_t)o * COUT, col, out_hi, out_lo, out_f32);
   }
   if (ovf && overflow) atomicOr(overflow, 1);
+}
+
+template <int COUT>
+__global__ void __launch_bounds__(256)
+spconv_first16_kernel(const float* __restrict__ feat_in, const int* __restrict__ nbr, const int* __restrict__ n_out_p,
+                      int out_cap, int c_in, int in_ld, int k_vol, const float* __restrict__ weight, Epi16 epi,
+                      __half* __restrict__ out_hi, __half* __restrict__ out_lo, float* __restrict__ out_f32,
+                      int* __restrict__ overflow) {
+  spconv_first16_body<COUT, 2>(feat_in, nbr, n_out_p, out_cap, c_in, in_ld, k_vol, weight, epi, out_hi, out_lo, out_f32,
+                               overflow);
+}
+
+// Single-pass FP16: writes the hi plane only.
+template <int COUT>
+__global__ void __launch_bounds__(256)
+spconv_first16_f16_kernel(const float* __restrict__ feat_in, const int* __restrict__ nbr, const int* __restrict__ n_out_p,
+                          int out_cap, int c_in, int in_ld, int k_vol, const float* __restrict__ weight, Epi16 epi,
+                          __half* __restrict__ out_hi, __half* __restrict__ out_lo, float* __restrict__ out_f32,
+                          int* __restrict__ overflow) {
+  spconv_first16_body<COUT, 1>(feat_in, nbr, n_out_p, out_cap, c_in, in_ld, k_vol, weight, epi, out_hi, out_lo, out_f32,
+                               overflow);
 }
 
 // ---- f16 weight image ------------------------------------------------------------------------------------------------
@@ -452,21 +520,25 @@ pack_weight16_kernel(const float* __restrict__ w, int c_in, int c_out, int k_vol
   }
 }
 
-// ---- plane <-> fp32 conversions (API boundary, tests) ------------------------------------------------------------------
+// ---- plane <-> fp32 conversions (API boundary, tests); PLANES = 1 reads / writes the hi plane alone -------------------
+template <int PLANES>
 __global__ void __launch_bounds__(256)
 split16_kernel(const float* __restrict__ x, long long n, __half* __restrict__ hi, __half* __restrict__ lo,
                int* __restrict__ overflow) {
   bool ovf = false;
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
-    ovf |= store16(x[e], hi + e, lo + e);
+    ovf |= store16p<PLANES>(x[e], hi + e, lo + e);
   }
   if (ovf && overflow) atomicOr(overflow, 1);
 }
 
+template <int PLANES>
 __global__ void __launch_bounds__(256)
 merge16_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo, long long n, float* __restrict__ x) {
-  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x)
-    x[e] = __half2float(hi[e]) + __half2float(lo[e]);
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
+    if constexpr (PLANES == 2) x[e] = __half2float(hi[e]) + __half2float(lo[e]);
+    else x[e] = __half2float(hi[e]);
+  }
 }
 
 // rows (f16 planes or fp32) -> channels-last BEV planes [B*H*W, C*D] (pre-zeroed), channel = c*D + z: the values of
@@ -475,7 +547,8 @@ merge16_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo, lon
 // the value is met, by the lowest lane of the lanes that meet one together: a per-thread flag carried to the end of the
 // grid-stride loop (as in split16_kernel) takes this kernel from 32 to 40 registers, and the PointPillars reader +
 // scatter stage (B = 8) from 0.191 to 0.201 ms in the replayed graph on an H100 80GB HBM3 at 700 W; this form keeps it
-// at 26 registers and 0.192 ms.
+// at 26 registers and 0.192 ms.  PLANES = 1 copies / rounds into the hi plane only.
+template <int PLANES>
 __global__ void __launch_bounds__(256)
 sparse_to_bev16_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ in_lo, const float* __restrict__ in_f32,
                        const int* __restrict__ coors, const int* __restrict__ n_rows, int row_cap, int C, int D, int H,
@@ -490,12 +563,12 @@ sparse_to_bev16_kernel(const __half* __restrict__ in_hi, const __half* __restric
       continue;
     const size_t dst = (((size_t)q.x * H + q.z) * W + q.w) * ((size_t)C * D) + (size_t)c * D + q.y;
     if (in_f32) {
-      if (store16(in_f32[e], out_hi + dst, out_lo + dst) && overflow) {
+      if (store16p<PLANES>(in_f32[e], out_hi + dst, out_lo + dst) && overflow) {
         if ((__activemask() & ((1u << (threadIdx.x & 31)) - 1u)) == 0u) atomicOr(overflow, 1);
       }
     } else {
       out_hi[dst] = in_hi[e];
-      out_lo[dst] = in_lo[e];
+      if constexpr (PLANES == 2) out_lo[dst] = in_lo[e];
     }
   }
 }
@@ -517,19 +590,20 @@ static Epi16 epi_of(const d3b_conv16_params* p) {
   return e;
 }
 
-template <int COUT>
+template <int COUT, int PLANES>
 static int launch_os16(const d3b_conv16_params* p, const int32_t* nbr, const uint32_t* tile_mask, const int32_t* n_out,
                        int32_t out_cap, cudaStream_t stream) {
-  using Cfg = OsCfg<COUT>;
+  using Cfg = OsCfg<COUT, PLANES>;
+  constexpr auto kernel = PLANES == 2 ? spconv_os16_kernel<COUT> : spconv_os16_f16_kernel<COUT>;
   static SmemOptIn optin;
-  D3B_CUDA(ensure_dynamic_smem(spconv_os16_kernel<COUT>, Cfg::kSmemBytes, optin));
+  D3B_CUDA(ensure_dynamic_smem(kernel, Cfg::kSmemBytes, optin));
   const int n_tiles = div_up(out_cap, kOsTileM);
   const int grid = n_tiles < kNumSMs ? (n_tiles > 0 ? n_tiles : 1) : kNumSMs;
   const int pack = os16_pack(p->c_in, p->k_vol);
   const int n_kb = pack > 1 ? 1 : (p->c_in + kOsKc - 1) / kOsKc;
   Epi16 epi = epi_of(p);
-  epi.corr = trunc_correction(p->c_in * pack);
-  D3B_CUDA(launch_maybe_pdl(spconv_os16_kernel<COUT>, dim3(grid), dim3(Cfg::kThreads), Cfg::kSmemBytes, stream,
+  epi.corr = trunc_correction(p->c_in * pack, PLANES == 2 ? 3 : 1);
+  D3B_CUDA(launch_maybe_pdl(kernel, dim3(grid), dim3(Cfg::kThreads), Cfg::kSmemBytes, stream,
                             (const __half*)p->in_hi, (const __half*)p->in_lo, (const int*)nbr, (const unsigned int*)tile_mask,
                             (const int*)n_out, (int)out_cap, (int)p->c_in, n_kb, pack, (int)p->k_vol,
                             (const __half*)p->weight_packed, epi,
@@ -538,16 +612,17 @@ static int launch_os16(const d3b_conv16_params* p, const int32_t* nbr, const uin
   return D3B_OK;
 }
 
-template <int COUT>
+template <int COUT, int PLANES>
 static int launch_first16(const d3b_conv16_params* p, const int32_t* nbr, const int32_t* n_out, int32_t out_cap,
                           cudaStream_t stream) {
+  constexpr auto kernel = PLANES == 2 ? spconv_first16_kernel<COUT> : spconv_first16_f16_kernel<COUT>;
   const size_t smem = (size_t)p->k_vol * p->c_in * COUT * sizeof(float);
   static SmemOptIn optin;
   D3B_REQUIRE(smem <= 160 * 1024, "first-layer sparse conv: weights (%zu bytes) do not fit in shared memory", smem);
-  D3B_CUDA(ensure_dynamic_smem(spconv_first16_kernel<COUT>, smem, optin));
+  D3B_CUDA(ensure_dynamic_smem(kernel, smem, optin));
   const int grid = grid_for((long long)out_cap * (COUT / 16) * 4, 256, 8);
   const int in_ld = p->in_f32_ld ? p->in_f32_ld : p->c_in;
-  spconv_first16_kernel<COUT><<<grid, 256, smem, stream>>>(p->in_f32, nbr, n_out, out_cap, p->c_in, in_ld, p->k_vol, p->weight,
+  kernel<<<grid, 256, smem, stream>>>(p->in_f32, nbr, n_out, out_cap, p->c_in, in_ld, p->k_vol, p->weight,
                                                          epi_of(p), (__half*)p->out_hi, (__half*)p->out_lo, p->out_f32,
                                                          p->overflow);
   D3B_LAUNCH_CHECK();
@@ -589,51 +664,61 @@ extern "C" int d3b_sparse_conv16(const int32_t* nbr, const uint32_t* tile_mask, 
   cudaStream_t stream = (cudaStream_t)stream_;
   D3B_REQUIRE(nbr && n_out && p, "d3b_sparse_conv16: null argument");
   D3B_REQUIRE(p->k_vol >= 1 && p->k_vol <= 32 && out_cap >= 0, "d3b_sparse_conv16: bad shape (k_vol %d)", p->k_vol);
-  D3B_REQUIRE((p->out_hi != nullptr) == (p->out_lo != nullptr) && (p->out_hi || p->out_f32),
-              "d3b_sparse_conv16: give out_hi + out_lo and/or out_f32");
+  D3B_REQUIRE(p->out_hi || p->out_f32, "d3b_sparse_conv16: give out_hi (+ out_lo) and/or out_f32");
   D3B_REQUIRE((p->scale == nullptr) == (p->shift == nullptr), "d3b_sparse_conv16: scale and shift go together");
-  D3B_REQUIRE((p->residual_hi == nullptr) == (p->residual_lo == nullptr), "d3b_sparse_conv16: residual planes go together");
+  PlanePairs pp;
+  pp.add(p->in_f32 ? nullptr : p->in_hi, p->in_lo);
+  pp.add(p->out_hi, p->out_lo);
+  pp.add(p->residual_hi, p->residual_lo);
+  D3B_REQUIRE(pp.consistent(),
+              "d3b_sparse_conv16: give in_lo, out_lo and residual_lo with their hi planes (FP16x3) or none of them "
+              "(single-pass FP16); got in_lo %s, out_lo %s, residual_lo %s",
+              p->in_lo ? "set" : "NULL", p->out_lo ? "set" : "NULL", p->residual_lo ? "set" : "NULL");
+  const bool two = pp.planes() == 2;
   if (out_cap == 0) return D3B_OK;
   if (p->in_f32) {      // first layer: fp32 rows, few channels
     D3B_REQUIRE(p->weight && p->c_in >= 1 && p->c_in <= 16, "d3b_sparse_conv16: fp32-input layers need weight and C_in <= 16");
     D3B_REQUIRE(p->in_f32_ld == 0 || p->in_f32_ld >= p->c_in, "d3b_sparse_conv16: in_f32_ld %d < C_in %d", p->in_f32_ld,
                 p->c_in);
     switch (p->c_out) {
-      case 16: return launch_first16<16>(p, nbr, n_out, out_cap, stream);
-      case 32: return launch_first16<32>(p, nbr, n_out, out_cap, stream);
-      case 64: return launch_first16<64>(p, nbr, n_out, out_cap, stream);
+      case 16: return two ? launch_first16<16, 2>(p, nbr, n_out, out_cap, stream) : launch_first16<16, 1>(p, nbr, n_out, out_cap, stream);
+      case 32: return two ? launch_first16<32, 2>(p, nbr, n_out, out_cap, stream) : launch_first16<32, 1>(p, nbr, n_out, out_cap, stream);
+      case 64: return two ? launch_first16<64, 2>(p, nbr, n_out, out_cap, stream) : launch_first16<64, 1>(p, nbr, n_out, out_cap, stream);
       default:
         set_error("d3b_sparse_conv16: fp32-input layer with C_out=%d (16/32/64 built)", p->c_out);
         return D3B_ERR_UNSUPPORTED;
     }
   }
-  D3B_REQUIRE(tile_mask && p->in_hi && p->in_lo && p->weight_packed, "d3b_sparse_conv16: null planes / tile_mask / packed weights");
+  D3B_REQUIRE(tile_mask && p->in_hi && p->weight_packed, "d3b_sparse_conv16: null planes / tile_mask / packed weights");
   if (!os16_shape_ok(p->c_in, p->c_out)) {
     set_error("d3b_sparse_conv16: unsupported C_in=%d C_out=%d", p->c_in, p->c_out);
     return D3B_ERR_UNSUPPORTED;
   }
   switch (p->c_out) {
-    case 16: return launch_os16<16>(p, nbr, tile_mask, n_out, out_cap, stream);
-    case 32: return launch_os16<32>(p, nbr, tile_mask, n_out, out_cap, stream);
-    case 64: return launch_os16<64>(p, nbr, tile_mask, n_out, out_cap, stream);
-    default: return launch_os16<128>(p, nbr, tile_mask, n_out, out_cap, stream);
+    case 16: return two ? launch_os16<16, 2>(p, nbr, tile_mask, n_out, out_cap, stream) : launch_os16<16, 1>(p, nbr, tile_mask, n_out, out_cap, stream);
+    case 32: return two ? launch_os16<32, 2>(p, nbr, tile_mask, n_out, out_cap, stream) : launch_os16<32, 1>(p, nbr, tile_mask, n_out, out_cap, stream);
+    case 64: return two ? launch_os16<64, 2>(p, nbr, tile_mask, n_out, out_cap, stream) : launch_os16<64, 1>(p, nbr, tile_mask, n_out, out_cap, stream);
+    default: return two ? launch_os16<128, 2>(p, nbr, tile_mask, n_out, out_cap, stream) : launch_os16<128, 1>(p, nbr, tile_mask, n_out, out_cap, stream);
   }
 }
 
+// lo == NULL: the single plane hi = f16(x) (split16), x = hi (merge16)
 extern "C" int d3b_split16(const float* x, int64_t n, void* hi, void* lo, int32_t* overflow, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  D3B_REQUIRE(n >= 0 && (n == 0 || (x && hi && lo)), "d3b_split16: null argument");
+  D3B_REQUIRE(n >= 0 && (n == 0 || (x && hi)), "d3b_split16: null argument");
   if (n == 0) return D3B_OK;
-  split16_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, n, (__half*)hi, (__half*)lo, overflow);
+  if (lo) split16_kernel<2><<<grid_for(n, 256), 256, 0, stream>>>(x, n, (__half*)hi, (__half*)lo, overflow);
+  else split16_kernel<1><<<grid_for(n, 256), 256, 0, stream>>>(x, n, (__half*)hi, nullptr, overflow);
   D3B_LAUNCH_CHECK();
   return D3B_OK;
 }
 
 extern "C" int d3b_merge16(const void* hi, const void* lo, int64_t n, float* x, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  D3B_REQUIRE(n >= 0 && (n == 0 || (x && hi && lo)), "d3b_merge16: null argument");
+  D3B_REQUIRE(n >= 0 && (n == 0 || (x && hi)), "d3b_merge16: null argument");
   if (n == 0) return D3B_OK;
-  merge16_kernel<<<grid_for(n, 256), 256, 0, stream>>>((const __half*)hi, (const __half*)lo, n, x);
+  if (lo) merge16_kernel<2><<<grid_for(n, 256), 256, 0, stream>>>((const __half*)hi, (const __half*)lo, n, x);
+  else merge16_kernel<1><<<grid_for(n, 256), 256, 0, stream>>>((const __half*)hi, nullptr, n, x);
   D3B_LAUNCH_CHECK();
   return D3B_OK;
 }
@@ -642,13 +727,25 @@ extern "C" int d3b_sparse_to_bev16(const void* in_hi, const void* in_lo, const f
                                    const int32_t* n_rows, int32_t row_cap, int32_t channels, const int32_t spatial[3],
                                    int32_t batch, void* out_hi, void* out_lo, int32_t* overflow, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  D3B_REQUIRE(coors && n_rows && spatial && out_hi && out_lo, "d3b_sparse_to_bev16: null argument");
-  D3B_REQUIRE((in_f32 != nullptr) != (in_hi != nullptr && in_lo != nullptr), "d3b_sparse_to_bev16: give fp32 rows OR both planes");
+  D3B_REQUIRE(coors && n_rows && spatial && out_hi, "d3b_sparse_to_bev16: null argument");
+  D3B_REQUIRE((in_f32 != nullptr) != (in_hi != nullptr), "d3b_sparse_to_bev16: give fp32 rows OR planes");
+  PlanePairs pp;
+  pp.add(in_hi, in_lo);
+  pp.add(out_hi, out_lo);
+  D3B_REQUIRE(pp.consistent(),
+              "d3b_sparse_to_bev16: give in_lo (plane rows) and out_lo together (FP16x3) or neither (single-pass FP16); "
+              "got in_lo %s, out_lo %s", in_lo ? "set" : "NULL", out_lo ? "set" : "NULL");
   D3B_REQUIRE(channels >= 1 && batch >= 1 && row_cap >= 0, "d3b_sparse_to_bev16: bad shape");
   if (row_cap == 0) return D3B_OK;
-  sparse_to_bev16_kernel<<<grid_for((long long)row_cap * channels, 256), 256, 0, stream>>>(
-      (const __half*)in_hi, (const __half*)in_lo, in_f32, coors, n_rows, row_cap, channels, spatial[0], spatial[1],
-      spatial[2], batch, (__half*)out_hi, (__half*)out_lo, overflow);
+  const int grid = grid_for((long long)row_cap * channels, 256);
+  if (pp.planes() == 2)
+    sparse_to_bev16_kernel<2><<<grid, 256, 0, stream>>>((const __half*)in_hi, (const __half*)in_lo, in_f32, coors, n_rows,
+                                                        row_cap, channels, spatial[0], spatial[1], spatial[2], batch,
+                                                        (__half*)out_hi, (__half*)out_lo, overflow);
+  else
+    sparse_to_bev16_kernel<1><<<grid, 256, 0, stream>>>((const __half*)in_hi, nullptr, in_f32, coors, n_rows, row_cap,
+                                                        channels, spatial[0], spatial[1], spatial[2], batch,
+                                                        (__half*)out_hi, nullptr, overflow);
   D3B_LAUNCH_CHECK();
   return D3B_OK;
 }

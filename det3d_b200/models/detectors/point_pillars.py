@@ -1,7 +1,7 @@
 """PointPillars detector (det3d/models/detectors/point_pillars.py:5-54): PillarFeatureNet reader ->
 PointPillarsScatter -> RPN -> MultiGroupHead."""
 from ..registry import DETECTORS
-from .voxelnet import SingleStageDetector, _FusedBevMixin
+from .voxelnet import F16_MATHS, SingleStageDetector, _FusedBevMixin
 
 
 @DETECTORS.register_module
@@ -29,12 +29,12 @@ class PointPillars(_FusedBevMixin, SingleStageDetector):
                     batch_size=len(num_voxels), input_shape=example["shape"][0], n_dev=example.get("n_voxels_dev"),
                     point_lists=example.get("point_lists"))
         bev = self.fused_bev() if not return_loss else None
-        if bev is not None and self.math == "fp16x3":
+        if bev is not None and self.math in F16_MATHS:
             kw = {} if data["n_dev"] is None else {"n_dev": data["n_dev"]}
             feats = self._read(data)
             ovf = self.overflow_flag(feats.device)
             planes = self.backbone.forward_planes(feats, data["coors"], data["batch_size"], data["input_shape"],
-                                                  overflow=ovf, **kw)
+                                                  overflow=ovf, n_planes=self.n_planes(), **kw)
             preds = bev.run(planes, overflow=ovf)
         else:
             preds = self.bbox_head(self.extract_feat(data))

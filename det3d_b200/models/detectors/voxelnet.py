@@ -6,6 +6,9 @@ from torch import nn
 from .. import builder
 from ..registry import DETECTORS
 
+MATHS = ("fp16x3", "fp16", "tf32x3")     # convolution arithmetic of the fused path (_FusedBevMixin.set_math)
+F16_MATHS = ("fp16x3", "fp16")           # the ones on f16 planes
+
 
 @DETECTORS.register_module
 class SingleStageDetector(nn.Module):
@@ -35,20 +38,28 @@ class _FusedBevMixin:
     """Routes RPN + heads through the det3d_b200 tensor-core kernels.
 
     math = "fp16x3" (default): NHWC split-f16 planes + TMA tensor maps (csrc/bevconv16_sm90.cu), any RPN the
-    reference builds; "tf32x3": the output-stationary 3xTF32 gather kernel over a dense rulebook (csrc/sparse_conv_sm90.cu,
-    stride-1 RPN only), which is also where a forward is re-run when a feature leaves the f16 range (`overflow_flag`)."""
+    reference builds; "fp16" (opt-in): the same kernels on the hi plane alone, one MMA per product -- faster, not
+    fp32-equivalent (DESIGN 3.0); "tf32x3": the output-stationary 3xTF32 gather kernel over a dense rulebook
+    (csrc/sparse_conv_sm90.cu, stride-1 RPN only), which is also where a forward is re-run when a feature leaves the f16
+    range (`overflow_flag`)."""
     use_fused_bev = True
     math = "fp16x3"
+    fp16_enabled = False        # set by det3d.core.fp16.wrap_fp16_model
     _bev16 = None
     _bev32 = None
     _ovf = None
 
     def set_math(self, math):
-        assert math in ("fp16x3", "tf32x3")
+        if math not in MATHS:
+            raise ValueError("unknown math %r: one of %s" % (math, ", ".join(MATHS)))
         self.math = math
         fused = getattr(self.backbone, "fused", None)
         if fused is not None:
             fused().math = math
+
+    def n_planes(self):
+        """f16 planes per activation on the fused path: 1 for "fp16", 2 for "fp16x3"."""
+        return 1 if self.math == "fp16" else 2
 
     def overflow_flag(self, device):
         # "cuda" (the pipeline's device) and "cuda:0" (a tensor's) must name the same flag: comparing them unresolved
@@ -65,7 +76,7 @@ class _FusedBevMixin:
         if self.training or not self.with_neck or not self.use_fused_bev:
             return None
         from det3d_b200.ops.spconv import bev
-        if self.math == "fp16x3":
+        if self.math in F16_MATHS:
             if self._bev16 is None:
                 ok = hasattr(self.backbone, "forward_planes") and bev.rpn_is_fusable16(self.neck)
                 self._bev16 = bev.FusedBevStack(self.neck, self.bbox_head) if ok else False
@@ -91,7 +102,7 @@ class VoxelNet(_FusedBevMixin, SingleStageDetector):
                     coors=example["coordinates"], batch_size=len(num_voxels),
                     input_shape=example["shape"][0], n_dev=example.get("n_voxels_dev"))
         bev = self.fused_bev() if not return_loss else None
-        if bev is not None and self.math == "fp16x3":
+        if bev is not None and self.math in F16_MATHS:
             feats = self.reader(data["features"], data["num_voxels"])
             ovf = self.overflow_flag(feats.device)
             planes = self.backbone.forward_planes(feats, data["coors"], data["batch_size"], data["input_shape"],

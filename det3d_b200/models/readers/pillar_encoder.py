@@ -165,10 +165,11 @@ class PointPillarsScatter(nn.Module):
     def init_weights(self, pretrained=None):
         pass
 
-    def forward_planes(self, voxel_features, coords, batch_size, input_shape, n_dev=None, overflow=None):
-        """[M, C] pillar features + coords -> NHWC split-f16 planes [B, ny, nx, C] (the FP16x3 dense path's input);
-        the canvas of pillar_encoder.py:175-211 in channels-last layout, split on the way.  A feature outside the f16
-        range ORs 1 into `overflow` (int32[1] device flag, or None)."""
+    def forward_planes(self, voxel_features, coords, batch_size, input_shape, n_dev=None, overflow=None, n_planes=2):
+        """[M, C] pillar features + coords -> NHWC split-f16 planes [B, ny, nx, C] (the FP16x3 dense path's input; with
+        n_planes = 1 the hi plane alone, for single-pass FP16); the canvas of pillar_encoder.py:175-211 in channels-last
+        layout, split on the way.  A feature outside the f16 range ORs 1 into `overflow` (int32[1] device flag, or
+        None)."""
         from det3d_b200.ops.spconv import conv16, core
         nx, ny = int(input_shape[0]), int(input_shape[1])
         feats = voxel_features.to(torch.float32).contiguous()
@@ -178,11 +179,11 @@ class PointPillarsScatter(nn.Module):
             n = torch.tensor([m, m], dtype=torch.int32, device=feats.device)
         else:
             n = torch.cat([n_dev.reshape(-1)[:1].to(torch.int32)] * 2)
-        key = (batch_size, ny, nx, feats.device)
+        key = (batch_size, ny, nx, feats.device, n_planes)
         cache = self.__dict__.setdefault("_planes", {})
         out = cache.get(key)
         if out is None:
-            out = cache[key] = conv16.Planes((batch_size, ny, nx, self.nchannels), feats.device)
+            out = cache[key] = conv16.Planes((batch_size, ny, nx, self.nchannels), feats.device, n_planes=n_planes)
         out.zero_()
         if m > 0:
             level = core.SparseLevel(coords, n, m, (1, ny, nx), batch_size)

@@ -258,7 +258,8 @@ def rpn_is_fusable16(rpn):
 
 
 class FusedBevStack:
-    """RPN + all task heads on NHWC f16 planes (FP16x3): one launch per conv layer, the deblocks write straight into
+    """RPN + all task heads on NHWC f16 planes (FP16x3, or single-pass FP16 when the input carries one plane: every
+    layer then runs on one plane, with the same packed weights): one launch per conv layer, the deblocks write straight into
     their channel slice of the concat buffer, and the heads of all tasks are ONE 1x1 conv whose fp32 output rows are
     already the NHWC-permuted layout `Head.forward` produces (mg_head.py:214-230)."""
 
@@ -311,10 +312,10 @@ class FusedBevStack:
         self._plan = dict(blocks=blocks, deblocks=deblocks, heads=heads, start=start,
                           concat=sum(d.c_out_total for d in deblocks))
 
-    def _planes(self, key, shape, device):
+    def _planes(self, key, shape, device, n_planes):
         p = self._bufs.get(key)
-        if p is None or p.shape != tuple(shape):
-            p = self._bufs[key] = conv16.Planes(shape, device)
+        if p is None or p.shape != tuple(shape) or p.n_planes != n_planes:
+            p = self._bufs[key] = conv16.Planes(shape, device, n_planes=n_planes)
         return p
 
     def layers(self):
@@ -337,13 +338,13 @@ class FusedBevStack:
                 self._compile(device)
                 self._sig = sig
             pl = self._plan
-            b = x.shape[0]
+            b, n_planes = x.shape[0], x.n_planes
             concat = None
             col = 0
             for i, blk in enumerate(pl["blocks"]):
                 for j, layer in enumerate(blk):
                     ho, wo = layer.out_hw(x.shape[1], x.shape[2])
-                    out = self._planes(("blk", i, j % 2), (b, ho, wo, layer.c_out_padded), device)
+                    out = self._planes(("blk", i, j % 2), (b, ho, wo, layer.c_out_padded), device, n_planes)
                     layer(x, out=out, overflow=overflow, tag="bev3x3" if layer.ksize == 3 else "bev1x1")
                     x = out
                 k = i - pl["start"]
@@ -351,7 +352,7 @@ class FusedBevStack:
                     de = pl["deblocks"][k]
                     ho, wo = de.out_hw(x.shape[1], x.shape[2])
                     if concat is None:
-                        concat = self._planes(("concat",), (b, ho, wo, pl["concat"]), device)
+                        concat = self._planes(("concat",), (b, ho, wo, pl["concat"]), device, n_planes)
                     assert tuple(concat.shape[1:3]) == (ho, wo), "deblock outputs must share one grid"
                     de(x, out=concat, out_c0=col, overflow=overflow, tag="deblock")
                     col += de.c_out_total

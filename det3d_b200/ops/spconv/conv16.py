@@ -1,7 +1,10 @@
-"""Split-f16 ("FP16x3") convolution primitives over the det3d_b200 C ABI (include/det3d_b200.h section 3b).
+"""Split-f16 ("FP16x3") and single-pass FP16 convolution primitives over the det3d_b200 C ABI (include/det3d_b200.h
+section 3b).
 
 An activation is carried as two f16 planes, hi = f16(x) and lo = f16(x - hi) (`Planes`); weights are split the same
-way after an exact power-of-two scaling.  `sparse_conv16` is the output-stationary sparse convolution
+way after an exact power-of-two scaling.  Single-pass FP16 carries the hi plane alone (`Planes(..., n_planes=1)`, whose
+`lo` is None): every entry point below then passes NULL lo pointers, which selects the kernels' one-MMA-per-product
+instantiations; the packed weight image is the same.  `sparse_conv16` is the output-stationary sparse convolution
 (csrc/spconv16_sm90.cu: deterministic, fused bias/BN/residual/ReLU epilogue), `BevConv16` a dense NHWC 3x3 / 1x1 /
 kernel = stride / ConvTranspose layer through TMA tensor maps (csrc/bevconv16_sm90.cu).
 
@@ -19,22 +22,25 @@ from ..._lib import Bev16Params, Conv16Params
 
 
 class Planes:
-    """hi / lo f16 planes of a [rows, C] (or [B, H, W, C]) activation: x = hi + lo to 22 significant bits."""
+    """hi / lo f16 planes of a [rows, C] (or [B, H, W, C]) activation: x = hi + lo to 22 significant bits.  With
+    n_planes = 1 (single-pass FP16) the hi plane alone, hi = f16(x), and `lo` is None."""
 
     __slots__ = ("buf", "shape")
 
-    def __init__(self, shape, device, zero=False):
+    def __init__(self, shape, device, zero=False, n_planes=2):
+        assert n_planes in (1, 2)
         self.shape = tuple(int(s) for s in shape)
         alloc = torch.zeros if zero else torch.empty
-        self.buf = alloc((2,) + self.shape, dtype=torch.float16, device=device)
+        self.buf = alloc((n_planes,) + self.shape, dtype=torch.float16, device=device)
 
+    n_planes = property(lambda self: self.buf.shape[0])
     hi = property(lambda self: self.buf[0])
-    lo = property(lambda self: self.buf[1])
+    lo = property(lambda self: self.buf[1] if self.buf.shape[0] == 2 else None)
     device = property(lambda self: self.buf.device)
 
     def view(self, *shape):
         p = Planes.__new__(Planes)
-        p.buf = self.buf.view((2,) + tuple(shape))
+        p.buf = self.buf.view((self.n_planes,) + tuple(shape))
         p.shape = tuple(p.buf.shape[1:])
         return p
 
@@ -43,11 +49,11 @@ class Planes:
         return self
 
     @staticmethod
-    def from_f32(x, overflow=None, out=None):
+    def from_f32(x, overflow=None, out=None, n_planes=2):
         x = x.contiguous().float()
-        p = out if out is not None else Planes(x.shape, x.device)
+        p = out if out is not None else Planes(x.shape, x.device, n_planes=n_planes)
         with _lib.on_device_of(x):
-            st = _lib.lib().d3b_split16(x.data_ptr(), x.numel(), p.hi.data_ptr(), p.lo.data_ptr(), _lib.ptr(overflow),
+            st = _lib.lib().d3b_split16(x.data_ptr(), x.numel(), p.hi.data_ptr(), _lib.ptr(p.lo), _lib.ptr(overflow),
                                         _lib.current_stream())
         _lib.check(st, "d3b_split16")
         return p
@@ -55,10 +61,15 @@ class Planes:
     def to_f32(self, out=None):
         x = out if out is not None else torch.empty(self.shape, dtype=torch.float32, device=self.device)
         with _lib.on_device_of(self.buf):
-            st = _lib.lib().d3b_merge16(self.hi.data_ptr(), self.lo.data_ptr(), x.numel(), x.data_ptr(),
+            st = _lib.lib().d3b_merge16(self.hi.data_ptr(), _lib.ptr(self.lo), x.numel(), x.data_ptr(),
                                         _lib.current_stream())
         _lib.check(st, "d3b_merge16")
         return x
+
+
+def math_of(planes):
+    """"fp16x3" for two planes, "fp16" for one (the label of a launch's stage timings)."""
+    return "fp16" if planes is not None and planes.n_planes == 1 else "fp16x3"
 
 
 def supported(c_in, c_out):
@@ -130,22 +141,23 @@ def sparse_conv16(x, rb, cw, out, residual=None, out_f32=None, overflow=None, ta
         dev_t = x
     else:
         assert isinstance(x, Planes) and x.shape[-1] == cw.c_in
-        p.in_hi, p.in_lo, p.weight_packed = x.hi.data_ptr(), x.lo.data_ptr(), cw.packed.data_ptr()
+        p.in_hi, p.in_lo, p.weight_packed = x.hi.data_ptr(), _lib.ptr(x.lo), cw.packed.data_ptr()
         dev_t = x.buf
     p.acc_scale = cw.acc_scale
     p.bias, p.scale, p.shift = _lib.ptr(cw.bias), _lib.ptr(cw.scale), _lib.ptr(cw.shift)
     if residual is not None:
         assert residual.shape[-1] == cw.c_out
-        p.residual_hi, p.residual_lo = residual.hi.data_ptr(), residual.lo.data_ptr()
+        p.residual_hi, p.residual_lo = residual.hi.data_ptr(), _lib.ptr(residual.lo)
     p.relu = 1 if cw.relu else 0
     if out is not None:
         assert out.shape[-1] == cw.c_out and out.shape[0] >= rb.out_level.cap
-        p.out_hi, p.out_lo = out.hi.data_ptr(), out.lo.data_ptr()
+        p.out_hi, p.out_lo = out.hi.data_ptr(), _lib.ptr(out.lo)
     if out_f32 is not None:
         assert out_f32.dtype == torch.float32 and out_f32.is_contiguous() and out_f32.shape[1] == cw.c_out
         p.out_f32 = out_f32.data_ptr()
     p.overflow = _lib.ptr(overflow)
-    with _lib.on_device_of(dev_t), _lib.timed(tag, c_in=cw.c_in, c_out=cw.c_out, k_vol=cw.k_vol, math="fp16x3"):
+    math = math_of(x if isinstance(x, Planes) else out)
+    with _lib.on_device_of(dev_t), _lib.timed(tag, c_in=cw.c_in, c_out=cw.c_out, k_vol=cw.k_vol, math=math):
         st = _lib.lib().d3b_sparse_conv16(rb.nbr.data_ptr(), rb.tile_mask.data_ptr(), rb.out_level.n.data_ptr(),
                                           rb.out_level.cap, C.byref(p), _lib.current_stream())
     _lib.check(st, "d3b_sparse_conv16")
@@ -154,18 +166,19 @@ def sparse_conv16(x, rb, cw, out, residual=None, out_f32=None, overflow=None, ta
 
 def sparse_to_bev16(x, level, out, overflow=None):
     """Sparse rows (Planes [cap, C] or fp32 [cap, C]) -> zero-filled NHWC planes `out` [B, H, W, C*D], channel = c*D+z.
-    fp32 rows are split on the way: one outside the f16 range ORs 1 into `overflow` (int32[1] device flag, or None)."""
+    fp32 rows are split on the way: one outside the f16 range ORs 1 into `overflow` (int32[1] device flag, or None).
+    Plane rows and `out` have the same plane count."""
     c = x.shape[-1]
     hi = lo = f32 = None
     if isinstance(x, Planes):
-        hi, lo, dev_t = x.hi.data_ptr(), x.lo.data_ptr(), x.buf
+        hi, lo, dev_t = x.hi.data_ptr(), _lib.ptr(x.lo), x.buf
     else:
         assert x.dtype == torch.float32 and x.is_contiguous()
         f32, dev_t = x.data_ptr(), x
     sp = (C.c_int32 * 3)(*[int(v) for v in level.spatial])
     with _lib.on_device_of(dev_t):
         st = _lib.lib().d3b_sparse_to_bev16(hi, lo, f32, level.coors.data_ptr(), level.n.data_ptr(), level.cap, c, sp,
-                                            level.batch, out.hi.data_ptr(), out.lo.data_ptr(), _lib.ptr(overflow),
+                                            level.batch, out.hi.data_ptr(), _lib.ptr(out.lo), _lib.ptr(overflow),
                                             _lib.current_stream())
     _lib.check(st, "d3b_sparse_to_bev16")
     return out
@@ -226,14 +239,15 @@ class BevConv16:
         return ho * self.up, wo * self.up
 
     def __call__(self, x, out=None, out_f32=None, out_c0=0, overflow=None, tag="bev"):
-        """x: Planes [B, H, W, C_in]; out: Planes [B, H', W', C_total] and/or out_f32 [B, H', W', C_total] fp32."""
+        """x: Planes [B, H, W, C_in]; out: Planes [B, H', W', C_total] (as many planes as x) and/or out_f32
+        [B, H', W', C_total] fp32.  One input plane runs the single-pass FP16 kernels."""
         b, h, w, c = x.shape
         assert c == self.c_in
         p = Bev16Params()
         p.batch, p.h_in, p.w_in, p.c_in = b, h, w, c
         p.c_out, p.ksize, p.stride, p.pad = self.c_blk, self.ksize, self.stride, self.pad
         p.groups, p.cgroups, p.up = self.groups, self.cgroups, self.up
-        p.in_hi, p.in_lo, p.weight_packed = x.hi.data_ptr(), x.lo.data_ptr(), self.packed.data_ptr()
+        p.in_hi, p.in_lo, p.weight_packed = x.hi.data_ptr(), _lib.ptr(x.lo), self.packed.data_ptr()
         p.acc_scale = self.acc_scale
         p.bias, p.scale, p.shift = _lib.ptr(self.bias), _lib.ptr(self.scale), _lib.ptr(self.shift)
         p.relu = 1 if self.relu else 0
@@ -249,7 +263,7 @@ class BevConv16:
                                                                         self.c_out_padded, p.out_c0,
                                                                         p.out_c0 + self.c_out_total, p.out_channels))
         if out is not None:
-            p.out_hi, p.out_lo = out.hi.data_ptr(), out.lo.data_ptr()
+            p.out_hi, p.out_lo = out.hi.data_ptr(), _lib.ptr(out.lo)
         if out_f32 is not None:
             assert out_f32.dtype == torch.float32 and out_f32.is_contiguous()
             if out is not None:
@@ -257,7 +271,7 @@ class BevConv16:
             p.out_f32 = out_f32.data_ptr()
         p.overflow = _lib.ptr(overflow)
         with _lib.on_device_of(x.buf), _lib.timed(tag, flops=self.flops(b, h, w), c_in=self.c_in, c_out=self.c_out_total,
-                                                  ksize=self.ksize, stride=self.stride, up=self.up, math="fp16x3",
+                                                  ksize=self.ksize, stride=self.stride, up=self.up, math=math_of(x),
                                                   pixels_in=b * h * w, pixels_out=b * ho * wo,
                                                   tiles=b * (-(-(ho // self.up) // 16)) * (-(-(wo // self.up) // 16)) * self.groups):
             st = _lib.lib().d3b_bev_conv16(C.byref(p), _lib.current_stream())

@@ -101,9 +101,10 @@ class FusedSparseEncoder:
     def __init__(self, middle_conv):
         self.plan = compile_plan(middle_conv)
         self._state = None
-        # "fp16x3" (default): output-stationary wgmma kernels on split-f16 planes (csrc/spconv16_sm90.cu).  "tf32x3":
+        # "fp16x3" (default): output-stationary wgmma kernels on split-f16 planes (csrc/spconv16_sm90.cu).  "fp16": the
+        # same kernels on the hi plane alone, one MMA per product (opt-in, not fp32-equivalent: DESIGN 3.0).  "tf32x3":
         # the output-stationary 3xTF32 kernels (csrc/sparse_conv_sm90.cu, SIMT where the shape is not built), the
-        # fallback when a feature leaves the f16 range.  Both are deterministic: fused epilogues, no atomics.
+        # fallback when a feature leaves the f16 range.  All are deterministic: fused epilogues, no atomics.
         self.math = "fp16x3"
         self.external_overflow = None   # int32[1] device flag shared with the rest of the model (else a private one)
         self.algo_override = None  # testing hook (tf32x3 path): force SIMT / TC for every layer
@@ -238,10 +239,10 @@ class FusedSparseEncoder:
         if (st is None or st["cap0"] < cap_needed or st["batch"] != batch_size
                 or st["spatial"] != tuple(spatial) or st["device"] != device):
             st = self._state = self._build_state(cap_needed, spatial, batch_size, device)
-        if self.math == "fp16x3" and self.algo_override is None:
+        if self.math in ("fp16x3", "fp16") and self.algo_override is None:
             return self._run16(st, features, coors, batch_size, n_dev, bev_rows)
         if bev_rows == "planes":
-            raise ValueError("BEV planes are produced by the fp16x3 path only")
+            raise ValueError("BEV planes are produced by the fp16x3 / fp16 paths only")
         self._refresh_weights(device)
         x = self._adopt_level0(st, features, coors, n_dev).contiguous()
         _side, before_conv = self._fork_rulebooks(st, device)
@@ -271,7 +272,11 @@ class FusedSparseEncoder:
         core.sparse_to_dense(x, st["final_level"], out=dense)
         return dense
 
-    # ---- FP16x3 path ------------------------------------------------------------------------
+    # ---- FP16x3 / single-pass FP16 path ---------------------------------------------------------
+    @property
+    def n_planes(self):
+        return 1 if self.math == "fp16" else 2
+
     def _refresh_weights16(self, device):
         for L in self.plan:
             sig = _signature(L)
@@ -285,10 +290,10 @@ class FusedSparseEncoder:
     def _bev_planes(self, st, batch_size, device):
         """NHWC f16 planes [B, H, W, C * D] of the encoder output (scn.py:192-195: dense.view(N, C * D, H, W))."""
         planes = st.get("bev_planes")
-        if planes is None or planes.shape[0] != batch_size:
+        if planes is None or planes.shape[0] != batch_size or planes.n_planes != self.n_planes:
             d, h, w = st["final_level"].spatial
             c = self.plan[-1].conv.out_channels
-            planes = st["bev_planes"] = conv16.Planes((batch_size, h, w, c * d), device)
+            planes = st["bev_planes"] = conv16.Planes((batch_size, h, w, c * d), device, n_planes=self.n_planes)
         return planes
 
     def overflowed(self):
@@ -322,14 +327,16 @@ class FusedSparseEncoder:
                 planes_cleared.record(side)
 
         first = self.plan[0].cw16
-        x = feats if first.fp32_input else conv16.Planes.from_f32(feats, ovf)
+        n_planes = self.n_planes
+        x = feats if first.fp32_input else conv16.Planes.from_f32(feats, ovf, n_planes=n_planes)
         identity = None
         for L, rb, build in st["steps"]:
             before_conv(rb, build)
             if L.save_identity:
                 identity = x
             cap, c = rb.out_level.cap, L.conv.out_channels
-            out = self._take(st["pools"], ("p16", cap, c), (x, identity), lambda: conv16.Planes((max(cap, 1), c), device))
+            out = self._take(st["pools"], ("p16", n_planes, cap, c), (x, identity),
+                             lambda: conv16.Planes((max(cap, 1), c), device, n_planes=n_planes))
             conv16.sparse_conv16(x, rb, L.cw16, out, residual=identity if L.residual else None, overflow=ovf)
             if L.residual:
                 identity = None
@@ -378,7 +385,7 @@ class FusedSparseEncoder:
             b = n_in * cin * 4 + n_out * cout * 4 + pairs * 8 + k * cin * cout * 4
             f = 2 * pairs * cin * cout
             layers.append(dict(n_in=n_in, n_out=n_out, pairs=pairs, c_in=cin, c_out=cout, k_vol=k, bytes=b, flops=f,
-                               algo="fp16x3" if L.cw is None else L.cw.algo))
+                               algo=self.math if L.cw is None else L.cw.algo))
             tot_b += b
             tot_f += f
         return dict(layers=layers, bytes=tot_b, flops=tot_f, dense_bytes=int(self._state["dense"].numel() * 4))

@@ -284,6 +284,14 @@ int d3b_rulebook_dense2d(int32_t batch, int32_t height, int32_t width, const int
  *     fp32 accumulation.  A result outside the f16 range cannot be carried: the kernels then OR 1 into `*overflow`
  *     (device int, may be NULL) and the caller must fall back to the tf32 path -- nothing saturates silently.
  *     Same reference call sites as section 3 (scn.py:106-157,323-355; necks/rpn.py:82-159; mg_head.py:198-230).
+ *
+ *     Single-pass FP16 (opt-in, not fp32-equivalent): a NULL lo plane selects it.  An activation is then the hi plane
+ *     alone, hi = f16(x), and the kernels compute hi.hi only (one MMA per product) from the same packed weight image;
+ *     the f16-range guard is the same.  The lo pointers of one call must all be given or all be NULL:
+ *       d3b_sparse_conv16 / d3b_bev_conv16: in_lo, out_lo (when out_hi is given) and residual_lo (when residual_hi is
+ *       given) -- e.g. in_lo set with out_lo NULL returns D3B_ERR_INVALID_ARG, with a message, before any CUDA call;
+ *       d3b_sparse_to_bev16: in_lo (with plane rows) and out_lo; d3b_split16 / d3b_merge16: lo.
+ *     A lo plane without its hi plane is rejected the same way.
  * ========================================================================= */
 typedef struct {
   int32_t c_in, c_out, k_vol;
@@ -299,7 +307,7 @@ typedef struct {
   const void* residual_hi;       /* f16 [rows, c_out] planes added before the ReLU, or NULL                     */
   const void* residual_lo;
   int32_t relu;
-  void* out_hi;                  /* f16 [rows, c_out] planes (both or neither)                                  */
+  void* out_hi;                  /* f16 [rows, c_out] planes (out_lo NULL: single-pass FP16, see above)         */
   void* out_lo;
   float* out_f32;                /* optional fp32 copy of the result [rows, c_out]                              */
   int32_t* overflow;             /* device flag, may be NULL                                                    */

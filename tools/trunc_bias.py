@@ -10,7 +10,9 @@ is printed with its standard error, in units of eps = 2^-26 (kTruncLossPerMma in
 (sparse output-stationary, dense pixel-stationary and pipelined) are measured against the split-exact result yh of the
 operands they see (tests/test_conv_error_model_gpu.py): each full slot chains n = 12 truncating MMAs and the epilogue
 adds 12 eps (kTruncLossPerMma per MMA) to the sums, so the true mean loss per MMA is about (12 eps - beta) / 12.  The tf32x3
-fallback kernels (simt, tc; tc over a dense rulebook) are measured against the exact y at features ~3e5.
+fallback kernels (simt, tc; tc over a dense rulebook) are measured against the exact y at features ~3e5.  The
+single-pass FP16 kernels (math "fp16") are measured against yh1 = sum a_hi w_hi (tests/test_fp16_single_gpu.py): a full
+slot chains n = 4 MMAs and the epilogue adds 4 eps.
 
     python tools/trunc_bias.py [--out FILE]
 """
@@ -27,6 +29,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch  # noqa: E402
 
 import test_conv_error_model_gpu as em  # noqa: E402
+import test_fp16_single_gpu as f1  # noqa: E402
 
 
 def gpu_info():
@@ -64,6 +67,21 @@ def tf32_case(algo, regime):
     return out, y
 
 
+def fp16_case(kernel, regime):
+    """The shapes of em.bias_case on the single-pass kernels -> (got, Ref1)."""
+    from det3d_b200 import _lib
+    if kernel == "sparse":
+        out, ref, *_ = f1.run_sparse1(64, 64, 27, 20000, 11, regime=regime, spatial=(20, 100, 100))
+        return out[:20000], ref
+    prev = _lib.lib().d3b_get_bev_variant()
+    try:
+        _lib.lib().d3b_set_bev_variant(2 if kernel == "dense_pl" else 0)
+        got, ref, *_ = f1.run_dense1(1, 96, 88, 128, 128, 3, 1, 1, 1, 23, regime=regime)
+    finally:
+        _lib.lib().d3b_set_bev_variant(prev)
+    return got, ref
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--out", default=None, help="also write the results as JSON lines to this file")
@@ -82,6 +100,13 @@ def main():
             applied = 12 * eps
             rows.append(dict(kernel=kernel, math="fp16x3", regime=regime, outputs=got.numel(), beta_eps=beta / eps,
                              se_eps=se / eps, applied_eps=applied / eps, loss_per_mma_eps=(applied - beta) / 12 / eps))
+    for kernel in ("sparse", "dense_ps", "dense_pl"):
+        for regime in ("A", "B", "C"):
+            got, ref = fp16_case(kernel, regime)
+            beta, se = em.residual_slope(got, ref.yh)
+            applied = 4 * eps
+            rows.append(dict(kernel=kernel, math="fp16", regime=regime, outputs=got.numel(), beta_eps=beta / eps,
+                             se_eps=se / eps, applied_eps=applied / eps, loss_per_mma_eps=(applied - beta) / 4 / eps))
     for algo in ("simt", "tc", "tc_dense"):
         for regime in ("A", "B", "C"):
             got, y = tf32_case(algo, regime)
@@ -90,7 +115,7 @@ def main():
                              se_eps=se / eps, beta_rel=beta))
     for r in rows:
         extra = (" (applied %+.0f eps/slot: loss/MMA %.2f eps)" % (r["applied_eps"], r["loss_per_mma_eps"])
-                 if r["math"] == "fp16x3" else " (%.2e relative)" % r["beta_rel"])
+                 if r["math"] in ("fp16x3", "fp16") else " (%.2e relative)" % r["beta_rel"])
         print("%-8s %-7s regime %s  n=%8d  beta = %+8.3f eps  se %.3f eps%s" % (
             r["kernel"], r["math"], r["regime"], r["outputs"], r["beta_eps"], r["se_eps"], extra))
     if args.out:
