@@ -119,3 +119,29 @@ def test_entry_points_validate_before_cuda_without_gpu():
     q = _lib.PredictParams()
     assert L.d3b_predict_workspace_bytes(ctypes.byref(q)) == 0
     assert L.d3b_predict_task(ctypes.byref(q), None, 0, 0, None, None, 0, None) == 1
+
+
+def test_pillar_reader_rejects_unbuilt_shapes_without_gpu():
+    """The pillar reader, both sources: every (ndim, units, max_points, batch) outside what the kernels are built for
+    returns its status and a message before any CUDA call -- 3 (unsupported) for ndim / units, 1 (invalid argument)
+    for sizes, a list-mode batch above 64, and staging above the 200 KB of shared memory."""
+    L = _lib.lib()
+    one = (ctypes.c_float * 8)()
+
+    def dense(rows, P, ndim, units):
+        return L.d3b_pillar_features(one, one, one, one, rows, P, ndim, units, one, one, one, 0.2, 0.2, 0.1, 0.1, one, None)
+
+    def lists(batch, P, ndim, units):
+        return L.d3b_pillar_features_lists(one, one, one, batch, 16, one, one, one, 4, P, ndim, units, one, one, one,
+                                           0.2, 0.2, 0.1, 0.1, one, None)
+
+    for call in (dense, lambda *a: lists(2, *a[1:])):
+        for ndim, units, status, word in ((12, 64, 3, b"ndim"), (4, 16, 3, b"units"), (4, 48, 3, b"units"),
+                                          (5, 160, 3, b"units"), (4, 64, 1, b"bad sizes")):
+            st = call(4, 0 if word == b"bad sizes" else 20, ndim, units)
+            assert st == status and word in L.d3b_last_error(), (ndim, units, st, L.d3b_last_error())
+        # (P, ndim) whose staging (4 warps x P x ndim fp32 + the weights) exceeds 200 KB
+        assert ((5 + 5) * 64 + 4 * 2600 * 5) * 4 > 200 * 1024
+        assert call(4, 2600, 5, 64) == 1 and b"shared memory" in L.d3b_last_error()
+    assert lists(65, 20, 4, 64) == 1 and b"batch 65" in L.d3b_last_error()
+    assert lists(0, 20, 4, 64) == 1 and b"batch 0" in L.d3b_last_error()
