@@ -19,10 +19,12 @@ import torch
 
 from det3d_b200 import _lib
 from det3d_b200.core.anchor.anchor_generator import anchors_for_tasks
+from det3d_b200.core.bbox.box_np_ops import camera_frustum_planes
 from det3d_b200.datasets.pipelines.loading import (MAX_BATCH, MAX_SWEEPS, BatchedIngest, SweepHistory,
                                                     check_sweep_samples, ingest_sweeps_batched, stage_raw_sweeps,
                                                     sweep_table_capacity)
 from det3d_b200.models import build_detector
+from det3d_b200.ops.point_cloud.frustum import MAX_NDIM, MIN_NDIM, FrustumCrop
 from det3d_b200.ops.point_cloud.voxelize import Voxelizer
 
 
@@ -52,10 +54,12 @@ class InferencePipeline:
         self.strict_fp32 = strict_fp32
         # (batch, bucket, ndim) -> _GraphEntry, (batch, raw bucket, table capacity, raw_stride, n_feat) ->
         # _SweepGraphEntry (infer_sweeps) and ("stream", B, K, slot_capacity, raw_stride, n_feat) -> _StreamGraphEntry
-        # (SweepStream.infer), least recently used first
+        # (SweepStream.infer) and ("frustum", B, raw bucket, ndim) -> _FrustumGraphEntry (infer_raw), least recently
+        # used first
         self._graphs = collections.OrderedDict()
         self.max_graphs = 8
         self._ovf_host = None
+        self._planes = collections.OrderedDict()      # calibration bytes -> frustum planes f64 [6, 4] (infer_raw)
 
     def anchors(self, batch):
         a = self._anchor_cache.get(batch)
@@ -296,6 +300,111 @@ class InferencePipeline:
                                                                    self.device))
         return entry
 
+    # ---- raw KITTI scans: camera-frustum crop on the device ----------------------------------------------------------
+    @staticmethod
+    def check_raw_clouds(clouds, calibs):
+        """Host-side validation of infer_raw's arguments: raises ValueError, before anything is enqueued.  Returns
+        (ndim, cloud sizes)."""
+        clouds, calibs = list(clouds), list(calibs)
+        if not 1 <= len(clouds) <= MAX_BATCH:
+            raise ValueError("a batch holds 1 to %d clouds, got %d" % (MAX_BATCH, len(clouds)))
+        if len(calibs) != len(clouds):
+            raise ValueError("%d clouds but %d calibrations" % (len(clouds), len(calibs)))
+        ndim, sizes = None, []
+        for b, c in enumerate(clouds):
+            if torch.is_tensor(c):
+                ok = c.dtype == torch.float32 and c.device.type == "cpu"
+            else:
+                ok = isinstance(c, np.ndarray) and c.dtype == np.float32
+            if not ok or c.ndim != 2:
+                raise ValueError("cloud %d: raw points must be a 2-D float32 host array" % b)
+            ndim = int(c.shape[1]) if ndim is None else ndim
+            if int(c.shape[1]) != ndim:
+                raise ValueError("cloud %d: %d columns, the batch has %d" % (b, c.shape[1], ndim))
+            sizes.append(int(c.shape[0]))
+        if not MIN_NDIM <= ndim <= MAX_NDIM:
+            raise ValueError("raw clouds must have %d to %d columns, got %d" % (MIN_NDIM, MAX_NDIM, ndim))
+        if sum(sizes) > 1 << 30:
+            raise ValueError("more than 2^30 raw points in one batch")
+        for b, cal in enumerate(calibs):
+            if not isinstance(cal, dict) or not all(k in cal for k in ("rect", "Trv2c", "P2", "image_shape")):
+                raise ValueError("calibration %d: expected dict(rect, Trv2c, P2, image_shape)" % b)
+            if np.shape(cal["rect"]) != (4, 4) or np.shape(cal["Trv2c"]) != (4, 4):
+                raise ValueError("calibration %d: rect and Trv2c must be 4x4 (the info files' extended form)" % b)
+            if np.shape(cal["P2"]) not in ((3, 4), (4, 4)):
+                raise ValueError("calibration %d: P2 must be 3x4 or 4x4, got shape %s" % (b, np.shape(cal["P2"])))
+            shape = np.asarray(cal["image_shape"]).reshape(-1)
+            if shape.shape[0] < 2 or not np.all(shape[:2] > 0):
+                raise ValueError("calibration %d: image_shape must be (H, W) > 0, got %r" % (b, cal["image_shape"]))
+        return ndim, sizes
+
+    def frustum_planes(self, calib):
+        """camera_frustum_planes of one calibration, cached by the calibration's bytes (KITTI calibrations change per
+        drive, not per frame)."""
+        # keyed on each matrix's dtype, shape and bytes: the planes are computed from the arrays as given, and numpy's
+        # inv / qr give a float32 calibration other planes than the same values in float64
+        parts = [np.ascontiguousarray(calib[k]) for k in ("rect", "Trv2c", "P2")]
+        shape = tuple(int(v) for v in np.asarray(calib["image_shape"]).reshape(-1)[:2])
+        key = b"".join(p.tobytes() for p in parts) + repr((shape, [(p.dtype.str, p.shape) for p in parts])).encode()
+        planes = self._planes.get(key)
+        if planes is None:
+            planes = camera_frustum_planes(calib["rect"], calib["Trv2c"], calib["P2"], shape)
+            self._planes[key] = planes
+            while len(self._planes) > 256:
+                self._planes.popitem(last=False)
+        else:
+            self._planes.move_to_end(key)
+        return planes
+
+    @torch.no_grad()
+    def infer_raw(self, clouds, calibs, pinned_out=None, graphed=False):
+        """Raw KITTI scans -> host detections [B, D, nd+3], as infer_host: each scan is first cropped to its camera's
+        view frustum (box_np_ops.remove_outside_points, bit-exact), on the device.
+
+        clouds: float32 [N_i, ndim] host arrays or tensors (pinned tensors are copied to the device directly), the full
+        360° scans; calibs[i]: dict(rect, Trv2c, P2, image_shape) -- res["calib"] plus the image shape (H, W).  One
+        d3b_frustum_crop_dev call crops the batch and writes the cropped clouds' device offsets, which the voxelizer
+        reads directly: no host sync before the D2H of the detections, which are the bits infer_host gives on the
+        cropped clouds.  graphed=True replays one CUDA graph covering crop, voxelize and forward per ("frustum", B,
+        raw bucket, ndim) (bucket_of of the raw total), in the LRU of forward_graphed; the scans are copied into its
+        static raw buffer, and the offsets and the plane table H2D only when they differ from that graph's last
+        replay.  The voxelizer's capacity is the raw bucket (the crop only removes points).  Raises ValueError before
+        anything is enqueued when the arguments are malformed.  The overflow fallback is infer_host's."""
+        clouds, calibs = list(clouds), list(calibs)
+        ndim, sizes = self.check_raw_clouds(clouds, calibs)
+        planes = np.stack([self.frustum_planes(c) for c in calibs])
+        offsets = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int32)
+        batch, bucket = len(clouds), self.bucket_of(int(offsets[-1]))
+        if not graphed:
+            crop = FrustumCrop(batch, bucket, ndim, self.device)
+            _stage_clouds(clouds, offsets, crop.points)
+            crop.set_table(offsets, planes)
+            points, cloud_offsets = crop.launch()
+        for _attempt in range(2):
+            if graphed:         # (a re-run after an overflow captures a new graph: check_overflow dropped them all)
+                entry = self._frustum_graph_entry(batch, bucket, ndim)
+                entry.stage(clouds, offsets, planes)
+                crop = entry.crop
+                packed = self._run_graph(entry, lambda: self.pack(self.forward_device(*crop.launch())))
+            else:
+                packed = self.pack(self.forward_device(points, cloud_offsets))
+            pinned_out, rerun = self._fetch(packed, pinned_out)
+            if not rerun:
+                break
+        return pinned_out
+
+    def _frustum_graph_entry(self, batch, bucket, ndim):
+        """The infer_raw graph of ("frustum", batch, bucket, ndim), in the LRU of forward_graphed."""
+        key = ("frustum", batch, bucket, ndim)
+        entry = self._graphs.get(key)
+        if entry is not None:
+            self._graphs.move_to_end(key)
+            return entry
+        while len(self._graphs) >= self.max_graphs:
+            self._graphs.popitem(last=False)
+        entry = self._graphs[key] = _FrustumGraphEntry(FrustumCrop(batch, bucket, ndim, self.device))
+        return entry
+
     @staticmethod
     def unpack(packed_host):
         """host [B, D, nd+3] -> list of dict(box3d_lidar, scores, label_preds) per sample."""
@@ -345,6 +454,57 @@ class _SweepGraphEntry:
         if self.raw_staging is None and not all(torch.is_tensor(r) and r.is_pinned() for s in samples for r in s[0]):
             self.raw_staging = torch.empty(self.ingest.raw.shape, dtype=torch.float32, pin_memory=True)
         stage_raw_sweeps(samples, sizes, self.ingest.raw, self.raw_staging)
+        self.copied.record()
+
+
+def _stage_clouds(clouds, offsets, points_dev, staging=None):
+    """Enqueues the H2D copies of the clouds into points_dev[offsets[b]:offsets[b + 1]].  Pinned tensors are copied
+    directly; anything else goes through the pinned `staging` buffer (allocated like points_dev when None).  Returns
+    the staging buffer."""
+    for c, a, b in zip(clouds, offsets[:-1], offsets[1:]):
+        if b > a:
+            src = c if torch.is_tensor(c) and c.is_pinned() else None
+            if src is None:
+                if staging is None:
+                    staging = torch.empty(points_dev.shape, dtype=torch.float32, pin_memory=True)
+                src = staging[a:b]
+                src.copy_(torch.as_tensor(c))
+            points_dev[a:b].copy_(src, non_blocking=True)
+    return staging
+
+
+class _FrustumGraphEntry:
+    """Static buffers of one captured infer_raw forward: the FrustumCrop (raw scans, offsets, planes, cropped clouds,
+    their offsets), the pinned staging of the offsets, of the planes and of scans that are not pinned already, the
+    graph and its output."""
+
+    def __init__(self, crop):
+        self.crop = crop
+        self.offsets_staging = torch.zeros(crop.offsets.shape, dtype=torch.int32, pin_memory=True)
+        self.planes_staging = torch.zeros(crop.planes.shape, dtype=torch.float64, pin_memory=True)
+        self.raw_staging = None
+        self.copied = torch.cuda.Event()
+        self.last_offsets = self.last_planes = None
+        self.planes_uploads = 0                   # plane-table H2D copies so far
+        self.graph = None
+        self.out = None
+
+    def stage(self, clouds, offsets, planes):
+        """Enqueue the H2D copies of the scans and, when they differ from the previous replay's, of the offsets and of
+        the plane table."""
+        # the pinned staging buffers may still feed the previous copies: wait for those before rewriting them
+        self.copied.synchronize()
+        crop = self.crop
+        if self.last_offsets is None or not np.array_equal(offsets, self.last_offsets):
+            self.offsets_staging.numpy()[:] = offsets
+            crop.offsets.copy_(self.offsets_staging, non_blocking=True)
+            self.last_offsets = offsets.copy()
+        if self.last_planes is None or not np.array_equal(planes.view(np.uint64), self.last_planes.view(np.uint64)):
+            self.planes_staging.numpy()[:] = planes
+            crop.planes.copy_(self.planes_staging, non_blocking=True)
+            self.last_planes = planes.copy()
+            self.planes_uploads += 1
+        self.raw_staging = _stage_clouds(clouds, offsets, crop.points, self.raw_staging)
         self.copied.record()
 
 

@@ -1,1 +1,1 @@
-from . import box_coders, box_torch_ops
+from . import box_coders, box_np_ops, box_torch_ops

@@ -20,9 +20,7 @@
 // d3b_ingest_sweeps_gather adds one device array, sweep_src: the raw row where each sweep starts, so sweeps can be read
 // from wherever they sit (a ring of history slots) while sweep_offsets stays the logical prefix that drives the chunks,
 // the scan and the cloud offsets.  Without it the start of sweep s is its offset, which is the other two entry points.
-#include <climits>
-
-#include "common.cuh"
+#include "chunk_scan.cuh"
 
 namespace d3b {
 namespace {
@@ -61,70 +59,17 @@ struct IngestTable {
   int buf[32];                                  // block-scan scratch
 };
 
-// Inclusive block-wide scan of one value per thread (sum, or max with kMax); `total` = the whole block's.  Every thread
-// of the block calls it; `buf` is 32 ints of shared memory, free again on return.
-template <bool kMax>
-__device__ __forceinline__ int block_scan(int v, int* buf, int& total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, v, d);
-    if (lane >= d) v = kMax ? max(v, t) : v + t;
-  }
-  if (lane == 31) buf[warp] = v;
-  __syncthreads();
-  if (warp == 0) {
-    int w = lane < (int)(blockDim.x >> 5) ? buf[lane] : (kMax ? INT_MIN : 0);
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, w, d);
-      if (lane >= d) w = kMax ? max(w, t) : w + t;
-    }
-    buf[lane] = w;
-  }
-  __syncthreads();
-  if (warp > 0) v = kMax ? max(v, buf[warp - 1]) : v + buf[warp - 1];
-  total = buf[31];
-  __syncthreads();
-  return v;
-}
-
-// dst[i] = min(max(0, raw(1..i)), cap) for i in [0, n] (dst[0] = 0): a table clamped into 0 = dst[0] <= ... <= dst[n]
-// <= cap.  With `chunks`, also chunks[i] = sum over j in [1, i] of ceil((dst[j] - dst[j-1]) / kIngestChunk).  Returns
-// (per thread) whether an entry it handled changed.
-template <class Raw>
-__device__ __forceinline__ bool clamp_table(Raw raw, int n, int cap, int* dst, int* chunks, int* buf) {
-  int run_max = 0, run_chunks = 0;
-  bool bad = false;
-  for (int base = 0; base <= n; base += blockDim.x) {
-    const int i = base + threadIdx.x;
-    const int r = i <= n ? raw(i) : 0;
-    int total;
-    const int m = max(block_scan<true>(i == 0 ? 0 : (i <= n ? r : INT_MIN), buf, total), run_max);
-    run_max = max(run_max, total);
-    const int c = min(m, cap);
-    bad |= i <= n && c != r;
-    if (i <= n) dst[i] = c;
-    if (chunks != nullptr) {
-      __syncthreads();
-      const int k = (i == 0 || i > n) ? 0 : (c - dst[i - 1] + kIngestChunk - 1) / kIngestChunk;
-      const int incl = block_scan<false>(k, buf, total) + run_chunks;
-      run_chunks += total;
-      if (i <= n) chunks[i] = incl;
-    }
-  }
-  return bad;
-}
-
 constexpr int kClampedTable = 1, kClampedSrc = 2;   // status bits
 
 // Fills `t` from the params (host table) or from device memory (device table, clamped).  Returns, to every thread after
 // the barrier, which clamps changed anything (kClampedTable | kClampedSrc).
 __device__ __forceinline__ int load_table(const IngestParams& p, IngestTable& t) {
-  bool bad = clamp_table([&](int i) { return p.off_dev != nullptr ? __ldg(p.off_dev + i) : p.off[i]; },
-                         p.n_sweeps, p.raw_cap, t.off, t.chunk_off, t.buf);
-  bad |= clamp_table([&](int b) { return p.sample_dev != nullptr ? __ldg(p.sample_dev + b) : (b == 0 ? 0 : p.n_sweeps); },
-                     p.batch, p.n_sweeps, t.sample, nullptr, t.buf);
+  bool bad = clamp_table<kIngestChunk>(
+      [&](int i) { return p.off_dev != nullptr ? __ldg(p.off_dev + i) : p.off[i]; }, p.n_sweeps, p.raw_cap, t.off,
+      t.chunk_off, t.buf);
+  bad |= clamp_table<kIngestChunk>(
+      [&](int b) { return p.sample_dev != nullptr ? __ldg(p.sample_dev + b) : (b == 0 ? 0 : p.n_sweeps); }, p.batch,
+      p.n_sweeps, t.sample, nullptr, t.buf);
   // t.off is complete here (the scans above passed barriers after writing it).  A gathered start is clamped into
   // [0, raw_cap - len]; without sweep_src the start is the offset itself, which is always inside.
   bool bad_src = false;
@@ -216,37 +161,7 @@ ingest_scan(const IngestParams p, const int* __restrict__ chunk_cnt, int* chunk_
   __shared__ int running;
   const int clamped = load_table(p, t);
   const int n_chunks = live_chunks(p, t);
-  int* warp_sums = t.buf;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) running = 0;
-  __syncthreads();
-  for (int base = 0; base < n_chunks; base += blockDim.x) {
-    const int g = base + threadIdx.x;
-    const int v = g < n_chunks ? chunk_cnt[g] : 0;
-    int incl = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl += t;
-    }
-    if (lane == 31) warp_sums[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      int w = warp_sums[lane];
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, w, d);
-        if (lane >= d) w += t;
-      }
-      warp_sums[lane] = w;
-    }
-    __syncthreads();
-    if (g < n_chunks) chunk_base[g] = running + (warp == 0 ? 0 : warp_sums[warp - 1]) + incl - v;
-    const int total = warp_sums[31];
-    __syncthreads();
-    if (threadIdx.x == 0) running += total;
-    __syncthreads();
-  }
+  scan_chunk_counts(chunk_cnt, n_chunks, chunk_base, t.buf, running);
   if (threadIdx.x == 0) {
     if (n_out != nullptr) *n_out = running < out_cap ? running : out_cap;
     if (status != nullptr) *status = clamped;

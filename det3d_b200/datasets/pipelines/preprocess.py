@@ -34,7 +34,8 @@ def _training_only(what):
 
 @PIPELINES.register_module
 class Preprocess(object):
-    """val/test behaviour of preprocess.py:28-257: pick the point array, optional shuffle, optional intensity shift."""
+    """val/test behaviour of preprocess.py:28-257: pick the point array, optional camera-frustum crop
+    (remove_outside_points, KITTI), optional shuffle, optional intensity shift."""
 
     def __init__(self, cfg=None, **kwargs):
         self.remove_environment = _get(cfg, "remove_environment", False)
@@ -47,8 +48,6 @@ class Preprocess(object):
             _training_only("Preprocess")
         if _get(cfg, "add_rgb_to_points", False) or _get(cfg, "reference_detections", None) is not None:
             raise NotImplementedError("Preprocess: add_rgb_to_points / reference_detections are unused by the configs in scope")
-        if self.remove_outside_points:
-            raise NotImplementedError("Preprocess: remove_outside_points needs the camera calibration path (out of scope)")
 
     def __call__(self, res, info):
         res["mode"] = self.mode
@@ -58,12 +57,35 @@ class Preprocess(object):
             points = res["lidar"]["combined"]
         else:
             raise NotImplementedError("Preprocess: dataset type %r" % (res["type"],))
+        if self.remove_outside_points:
+            points = self._remove_outside_points(res, points)
         if self.shuffle_points:
             np.random.shuffle(points)                       # preprocess.py:213-215 (in place, same RNG stream)
         if self.symmetry_intensity:
             points[:, -1] -= 0.5                            # :248-250
         res["lidar"]["points"] = points
         return res, info
+
+    @staticmethod
+    def _remove_outside_points(res, points):
+        """preprocess.py:111-116: keep the points inside the camera's view frustum (box_np_ops.remove_outside_points,
+        on the device), from res["calib"] (rect, Trv2c, P2, as LoadPointCloudAnnotations fills it for a KittiDataset)
+        and the image shape.  The reference reads the shape from res["image"]["image_shape"], which its own
+        KittiDataset.get_sensor_data (kitti.py:206-222) never sets; here res["image"] is read when present, else
+        res["metadata"]["image_shape"].  Raises ValueError without a calibration (the reference's
+        `assert calib is not None`), so for every dataset but KITTI."""
+        from det3d_b200.core.bbox import box_np_ops
+
+        calib = res.get("calib")
+        if calib is None:
+            raise ValueError("Preprocess: remove_outside_points needs res['calib'] (a KittiDataset with "
+                             "LoadPointCloudAnnotations), %s has none" % (res["type"],))
+        image = res.get("image")
+        if image is not None and "image_shape" in image:
+            image_shape = image["image_shape"]
+        else:
+            image_shape = res["metadata"]["image_shape"]
+        return box_np_ops.remove_outside_points(points, calib["rect"], calib["Trv2c"], calib["P2"], image_shape)
 
 
 @PIPELINES.register_module

@@ -1,2 +1,3 @@
 from .point_cloud_ops import points_to_voxel
 from .voxelize import Voxelizer, grid_size_of
+from .frustum import FrustumCrop

@@ -243,3 +243,58 @@ def calibrate_demo_weights_(model, cfg, clouds, seed=0, pass_fraction=0.03, box_
         for h in hooks:
             h.remove()
     return model
+
+
+def raw_velodyne_scan(n=120000, ndim=4, seed=0, max_range=120.0):
+    """A full 360° scan of a 64-beam spinning LiDAR, KITTI-style: no range or field-of-view crop, ordered beam by beam
+    and by azimuth within a beam (as a raw velodyne file).  Beams at -24.8° .. +2° elevation from 1.73 m above the
+    ground hit the ground or (35 %) an obstacle at 2 m .. max_range; rays that hit nothing within max_range are dropped,
+    so the scan holds about n points (n / 64 azimuth steps per beam)."""
+    rng = np.random.default_rng(seed)
+    per_beam = max(int(n) // 64, 1)
+    beam = np.repeat(np.arange(64), per_beam)
+    elev = np.deg2rad(-24.8 + beam * (26.8 / 63.0)) + rng.normal(0, 1e-3, beam.shape[0])
+    azim = np.tile(np.linspace(-np.pi, np.pi, per_beam, endpoint=False), 64) + rng.normal(0, 1e-4, beam.shape[0])
+    h = 1.73
+    with np.errstate(divide="ignore"):
+        ground_d = np.where(elev < -1e-3, h / np.tan(-elev), np.inf)
+    obst = rng.uniform(0, 1, beam.shape[0]) < 0.35
+    obst_d = rng.uniform(2.0, max_range, beam.shape[0])
+    d = np.where(obst, np.minimum(obst_d, ground_d), ground_d)
+    ok = d < max_range
+    z = -h + np.where(obst & (obst_d < ground_d), rng.uniform(0, 2.5, beam.shape[0]), 0.0) + rng.normal(0, 0.02, beam.shape[0])
+    pts = np.zeros((int(ok.sum()), ndim), np.float32)
+    pts[:, 0], pts[:, 1], pts[:, 2] = (d * np.cos(azim))[ok], (d * np.sin(azim))[ok], z[ok]
+    if ndim > 3:
+        pts[:, 3] = rng.uniform(0, 1, pts.shape[0])
+    return pts
+
+
+KITTI_IMAGE_SHAPES = ((375, 1242), (370, 1224), (374, 1238), (376, 1241))
+
+
+def kitti_like_calib(seed=0, image_shape=(375, 1242), perturb=True):
+    """A synthetic KITTI calibration in the info files' form: dict(rect, Trv2c, P2, image_shape), 4x4 float64 matrices.
+    P2 = K [I | t] with KITTI-like intrinsics (f ≈ 721.5, c ≈ (609.6, 172.9)) and P2[:, 3] ≈ (44.86, 0.216, 0.0027);
+    R0_rect a small rotation; Tr_velo_to_cam the velodyne -> camera axis permutation times a small rotation, plus a
+    translation of about (-0.004, -0.076, -0.27).  `perturb` adds seeded jitter to every parameter."""
+    rng = np.random.default_rng(seed)
+    j = (lambda s: rng.normal(0, s)) if perturb else (lambda s: 0.0)
+
+    def rot(ax, ay, az):
+        cx, sx, cy, sy, cz, sz = np.cos(ax), np.sin(ax), np.cos(ay), np.sin(ay), np.cos(az), np.sin(az)
+        return (np.array([[cz, -sz, 0], [sz, cz, 0], [0, 0, 1]]) @ np.array([[cy, 0, sy], [0, 1, 0], [-sy, 0, cy]])
+                @ np.array([[1, 0, 0], [0, cx, -sx], [0, sx, cx]]))
+
+    f = 721.5377 * (1 + j(0.01))
+    K = np.array([[f, 0, 609.5593 + j(3.0)], [0, f, 172.854 + j(3.0)], [0, 0, 1.0]])
+    t = np.linalg.solve(K, np.array([44.85728 + j(0.5), 0.2163791 + j(0.01), 0.002745884 + j(1e-4)]))
+    P2 = np.eye(4)
+    P2[:3, :3], P2[:3, 3] = K, K @ t
+    rect = np.eye(4)
+    rect[:3, :3] = rot(0.0042 + j(0.002), -0.0099 + j(0.002), 0.0074 + j(0.002))
+    axes = np.array([[0, -1.0, 0], [0, 0, -1.0], [1.0, 0, 0]])             # velodyne x fwd, y left, z up -> camera
+    Trv2c = np.eye(4)
+    Trv2c[:3, :3] = axes @ rot(j(0.01), j(0.01), j(0.01))
+    Trv2c[:3, 3] = [-0.004069766 + j(0.002), -0.07631618 + j(0.005), -0.2717806 + j(0.01)]
+    return dict(rect=rect, Trv2c=Trv2c, P2=P2, image_shape=np.array(image_shape, np.int64))

@@ -151,6 +151,31 @@ int d3b_ingest_sweeps_gather(const float* raw, int32_t raw_capacity, int32_t raw
                              int32_t sweep_capacity, int32_t batch, float radius, float* out, int32_t* cloud_offsets,
                              int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
 
+/* KITTI camera-frustum crop for a batch of raw scans, with the cloud offsets and the planes in DEVICE memory, for graph
+ * replay over scans of any size.  replaces box_np_ops.remove_outside_points (det3d/core/bbox/box_np_ops.py:941-952;
+ * the point test of core/bbox/geometry.py:241-276) as called by Preprocess (datasets/pipelines/preprocess.py:111-116).
+ * 1 <= batch <= 64, 3 <= ndim <= 16.
+ * points            [point_capacity, ndim] f32 device: the scans back to back; rows at or past cloud_offsets_in[batch]
+ *                   are never read
+ * cloud_offsets_in  [batch + 1] i32 DEVICE: scan b is rows [off[b], off[b + 1])
+ * planes            [batch][6][4] f64 DEVICE: scan b's frustum planes (n0, n1, n2, d), in the reference's order
+ *                   (det3d_b200.core.bbox.box_np_ops.camera_frustum_planes).  A point is kept when every plane gives
+ *                   s = ((x*n0 + y*n1) + z*n2) + d < 0, x, y, z promoted to f64, each operation rounded on its own (no
+ *                   FMA); a NaN coordinate fails every s >= 0 test and is kept, as in the reference
+ * out               [point_capacity, ndim] f32 device: the kept rows of every scan (all ndim columns), scan after scan,
+ *                   each in input order
+ * cloud_offsets_out [batch + 1] i32 device: scan b's kept rows are [cloud_offsets_out[b], cloud_offsets_out[b + 1]) of
+ *                   `out` -- the form d3b_voxelize_dev takes
+ * status            [1] i32 device or NULL: set to 1 if the offsets were not 0 = off[0] <= ... <= off[batch] <=
+ *                   point_capacity; they are then clamped into that shape as off[i] = min(max(0, off[1..i]),
+ *                   point_capacity) before any point index is formed (0 when they were)
+ * workspace: d3b_frustum_crop_workspace_bytes(point_capacity, batch) (0 for arguments out of range).  Runs three kernels
+ * (count, scan, emit), no host sync; each scan's rows are bit-identical to that scan cropped alone. */
+size_t d3b_frustum_crop_workspace_bytes(int32_t point_capacity, int32_t batch);
+int d3b_frustum_crop_dev(const float* points, int32_t point_capacity, int32_t ndim, const int32_t* cloud_offsets_in,
+                         const double* planes, int32_t batch, float* out, int32_t* cloud_offsets_out, int32_t* status,
+                         void* workspace, size_t workspace_bytes, void* stream);
+
 /* ========================================================================= *
  * 2. Rulebook (sparse-convolution index maps)
  *    replaces spconv v1.x `get_indice_pairs` as called by SubMConv3d /
