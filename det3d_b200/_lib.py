@@ -147,6 +147,8 @@ SIGNATURES = {
     "d3b_merge16": (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
     "d3b_sparse_to_bev16": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _I3, _i32, _vp, _vp, _vp, _vp]),
     "d3b_bev_conv16": (C.c_int, [C.POINTER(Bev16Params), _vp]),
+    "d3b_bev_conv16_chain_workspace_bytes": (_i64, [_i32, _i32, _i32, _i32]),
+    "d3b_bev_conv16_chain": (C.c_int, [C.POINTER(Bev16Params), _i32, _vp, _i64, _vp]),
     "d3b_predict_workspace_bytes": (_sz, [C.POINTER(PredictParams)]),
     "d3b_predict_task": (C.c_int, [C.POINTER(PredictParams), _vp, _i32, _i32, _vp, _vp, _sz, _vp]),
     "d3b_boxes_iou_bev": (C.c_int, [_vp, _i32, _vp, _i32, _i32, _vp, _vp]),

@@ -290,8 +290,8 @@ bev_conv16_f16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_co
 // one m64n128k16 chain into one of two 64-register partials: slot s is issued into P[s & 1] while slot s - 1 is still
 // running, then `wait_group 1` and s - 1 is folded.  Sums + two partials fit the 232 registers the consumer warpgroups
 // take with setmaxnreg (the producer warpgroup keeps 40), so nothing spills and the tensor pipe always has the next slot
-// queued.  The small tile also balances the grid: SECOND's 200 x 176 plane is 286 tiles (3 rounds of 128 pixels on
-// 132 SMs) instead of 143 (2 rounds of 256).  Same products, same order, same fold, same correction and epilogue as
+// queued.  Within one layer no tile size the register budget allows fills the grid (SECOND's 200 x 176 plane is 286
+// tiles: 3 rounds of the 132 SMs, the last with 22 CTAs); chaining the layers of a block (below) does.  Same products, same order, same fold, same correction and epilogue as
 // the pixel-stationary kernel: bit-identical to it.
 //  * A stage = one box per plane, 64 channels x 8 pixels x 18 rows (18 KB); block m reads kernel row ky at
 //    m * 8192 + ky * 1024.  B stage = [W_hi | W_lo] of one (kb, kx, ky).  Three stages of each.
@@ -309,13 +309,82 @@ struct PlCfg {
 constexpr int kPlConsumerRegs = 232, kPlProducerRegs = 40;        // 2 * 232 + 40 <= 512 per thread triple
 static_assert(2 * kPlConsumerRegs + kPlProducerRegs <= 512, "register budget of one SM");
 
+// Chains of 3x3 stride-1 layers (d3b_bev_conv16_chain): one persistent launch runs up to kPlMaxLayers layers of one
+// grid, handing out the tiles of every layer in order.  A tile of layer l + 1 reads only the 3 x 3 neighbourhood of
+// tiles layer l wrote, so it can start while layer l is still finishing elsewhere: SECOND's six 286-tile layers run as
+// 1716 tiles = 13 rounds of the 132 SMs instead of 6 x 3, and there are no launch boundaries in between.
+//  * Work list: ticket t -> (layer, sample, tile, output group), layer-major, the output groups of a tile next to each
+//    other.  One global counter hands the tickets out; the producer's elected lane fetches one per tile and passes it
+//    to the consumer warpgroups through a two-entry shared ring.  Without a workspace (d3b_bev_conv16, one layer) the
+//    producer walks t = blockIdx.x, += gridDim.x instead.
+//  * Dependencies: done[l][sample][tile] counts the output groups of a layer-l tile whose planes are written (the 256
+//    consumer threads fence their stores to the async proxy, meet at a named barrier, and one thread adds with release
+//    semantics).  Before the first A load of a layer-l tile (l >= 1) the producer polls, with acquire semantics, the
+//    <= 9 neighbouring tiles of layer l - 1 until each counts all of that layer's groups, then fences to the async
+//    proxy: the planes were written through the generic proxy and TMA reads them through the async one.
+//  * No deadlock: a ticket only waits on smaller tickets, and every smaller ticket was claimed by a CTA that is already
+//    running and has issued (or is issuing) all of that ticket's loads before it fetches another -- so the smallest
+//    unfinished ticket can always progress, whether or not all CTAs are co-resident.
+//  * Buffer reuse: the stacks ping-pong two buffers, so layer l + 1 overwrites what layer l - 1 wrote and layer l read.
+//    Layer-l tiles that read the region of tile i are exactly the neighbours of i that the layer-(l + 1) tile i waits
+//    on, and a tile counts as done only after its consumers have used every staged patch: the read-after-write wait
+//    also covers the write-after-read hazard (transitively for any older layer).  The host requires layer k's input to
+//    be layer k - 1's output and no layer to write its own input.
+//  * Replay: the last CTA to leave (a second counter) sets the ticket counter and the done counters back to zero, so
+//    a replayed graph needs no host action and no extra node.
+constexpr int kPlMaxLayers = 8;
+struct PlLayer {
+  CUtensorMap tm_hi, tm_lo;
+  BvGeom g;                       // tiles_x counts 8-column tiles
+  const __half* packed;
+  Epi16 epi;
+  __half* out_hi;
+  __half* out_lo;
+  float* out_f32;
+};
+struct PlChain {
+  PlLayer layer[kPlMaxLayers];
+  int n_layers;
+  int first_ticket[kPlMaxLayers + 1];   // layer l's tickets are [first_ticket[l], first_ticket[l + 1])
+  int spatial;                          // tiles of one layer and output group: batch * tiles_y * tiles_x
+  int seq;                              // launch counter (development traces only)
+  int* overflow;
+  unsigned int* work;                   // null: static walk; else [0] tickets, [1] CTAs done, [2 + l * spatial + s] done
+};
+static_assert(sizeof(PlChain) <= 4096, "chain parameters must fit the classic 4 KB kernel-parameter space");
+
+__device__ __forceinline__ unsigned int ld_acquire_gpu(const unsigned int* p) {
+  unsigned int v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void red_release_gpu_add(unsigned int* p, unsigned int v) {
+  asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+
+// Waits until done[i] == want (bounded: a protocol bug traps instead of hanging the GPU; the development library
+// records code 6 in the fault word and returns).
+__device__ __forceinline__ void wait_done(const unsigned int* done, unsigned int want) {
+  for (uint32_t spin = 0; ld_acquire_gpu(done) != want; ++spin) {
+#ifdef D3B_SOFT_TIMEOUT
+    if (spin > (1u << 20)) {
+      const unsigned int slot = atomicAdd(&g_d3b_fault[0], 1u);
+      if (slot < 7u) g_d3b_fault[1 + slot] = (6u << 16) | (blockIdx.x & 0xffffu);
+      return;
+    }
+#else
+    if (spin > (1u << 26)) __trap();
+#endif
+  }
+}
+
 template <int PLANES>
-__device__ __forceinline__ void bev_conv16_pl_body(const CUtensorMap* tm_hi, const CUtensorMap* tm_lo, const BvGeom& g,
-                                                   const __half* __restrict__ packed, const Epi16& epi,
-                                                   __half* __restrict__ out_hi, __half* __restrict__ out_lo,
-                                                   float* __restrict__ out_f32, int* __restrict__ overflow) {
+__device__ __forceinline__ void bev_conv16_pl_body(const PlChain& P) {
   constexpr int kPlAStageBytes = PlCfg<PLANES>::kAStageBytes, kPlBBytes = PlCfg<PLANES>::kBBytes;
   extern __shared__ uint8_t smem_raw[];
+  __shared__ int tk_ring[2];
+  __shared__ int last_cta;
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_base = smem_base;
   const uint32_t b_base = a_base + kPlStages * kPlAStageBytes;
@@ -324,33 +393,42 @@ __device__ __forceinline__ void bev_conv16_pl_body(const CUtensorMap* tm_hi, con
   auto a_empty = [&](uint32_t s) { return bar_base + 8u * (kPlStages + s); };
   auto b_full = [&](uint32_t s) { return bar_base + 8u * (2 * kPlStages + s); };
   auto b_empty = [&](uint32_t s) { return bar_base + 8u * (3 * kPlStages + s); };
+  auto tk_full = [&](uint32_t s) { return bar_base + 8u * (4 * kPlStages + s); };
+  auto tk_empty = [&](uint32_t s) { return bar_base + 8u * (4 * kPlStages + 2 + s); };
 
-  D3B_CTA_MARK(0, epi.seq);
+  D3B_CTA_MARK(0, P.seq);
   pdl_launch_dependents();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tiles_per_group = g.batch * g.tiles_y * g.tiles_x;     // tiles_x counts 8-column tiles here
-  const int n_tiles = tiles_per_group * g.groups;
-  const int n_slots = 9 * g.n_kb;                                  // (kb, kx, ky), ky fastest
+  const int n_tickets = P.first_ticket[P.n_layers];
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kPlStages; ++s) {
       mbar_init(a_full(s), 1); mbar_init(a_empty(s), kBvMathWarps);
       mbar_init(b_full(s), 1); mbar_init(b_empty(s), kBvMathWarps);
     }
+    for (int s = 0; s < 2; ++s) { mbar_init(tk_full(s), 1); mbar_init(tk_empty(s), kBvMathWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    tma_prefetch_desc(tm_hi);
-    if constexpr (PLANES == 2) tma_prefetch_desc(tm_lo);
+    for (int l = 0; l < P.n_layers; ++l) {
+      tma_prefetch_desc(&P.layer[l].tm_hi);
+      if constexpr (PLANES == 2) tma_prefetch_desc(&P.layer[l].tm_lo);
+    }
   }
   __syncthreads();
   pdl_wait_prior_grid();             // everything below reads the previous layer's planes or writes buffers it may still read
 
-  auto decode = [&](int tile, int& grp, int& b, int& y0, int& x0) {
-    grp = tile / tiles_per_group;
-    int t = tile - grp * tiles_per_group;
-    b = t / (g.tiles_y * g.tiles_x);
-    t -= b * g.tiles_y * g.tiles_x;
-    y0 = (t / g.tiles_x) * kBvTileY;
-    x0 = (t % g.tiles_x) * kBvHalfX;
+  // ticket -> (layer, output group, sample, y0, x0, tile index within the layer's grid)
+  auto decode = [&](int t, int& l, int& grp, int& b, int& y0, int& x0, int& sp) {
+    l = 0;
+    while (l + 1 < P.n_layers && t >= P.first_ticket[l + 1]) ++l;
+    const BvGeom& g = P.layer[l].g;
+    const int u = t - P.first_ticket[l];
+    grp = u % g.groups;
+    sp = u / g.groups;
+    const int per_sample = g.tiles_y * g.tiles_x;
+    b = sp / per_sample;
+    const int r = sp - b * per_sample;
+    y0 = (r / g.tiles_x) * kBvTileY;
+    x0 = (r % g.tiles_x) * kBvHalfX;
   };
 
   if (warp >= kBvTmaWarp) {
@@ -358,28 +436,46 @@ __device__ __forceinline__ void bev_conv16_pl_body(const CUtensorMap* tm_hi, con
     regs_dealloc<kPlProducerRegs>();
     if (warp == kBvTmaWarp && lane == 0) {
       uint32_t a_it = 0, b_it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        int grp, b, y0, x0;
-        decode(tile, grp, b, y0, x0);
-        const __half* wgrp = packed + (size_t)grp * 9 * g.n_kb * kPlSlotHalves;
-        for (int kb = 0; kb < g.n_kb; ++kb) {
+      int t = blockIdx.x;
+      for (uint32_t it = 0;; ++it) {
+        const uint32_t s = it & 1u;
+        D3B_WAIT(tk_empty(s), ((it >> 1) & 1u) ^ 1u, 7);
+        if (P.work) t = (int)atomicAdd(P.work, 1u);
+        tk_ring[s] = t;
+        mbar_arrive(tk_full(s));
+        if (t >= n_tickets) break;
+        int l, grp, b, y0, x0, sp;
+        decode(t, l, grp, b, y0, x0, sp);
+        const PlLayer& L = P.layer[l];
+        if (P.work && l > 0) {
+          const BvGeom& gp = P.layer[l - 1].g;
+          const unsigned int* done = P.work + 2 + (size_t)(l - 1) * P.spatial + b * gp.tiles_y * gp.tiles_x;
+          const int ty = y0 / kBvTileY, tx = x0 / kBvHalfX;
+          for (int y = max(ty - 1, 0); y <= min(ty + 1, gp.tiles_y - 1); ++y)
+            for (int x = max(tx - 1, 0); x <= min(tx + 1, gp.tiles_x - 1); ++x)
+              wait_done(done + y * gp.tiles_x + x, (unsigned int)gp.groups);
+          fence_proxy_async_global();
+        }
+        const __half* wgrp = L.packed + (size_t)grp * 9 * L.g.n_kb * kPlSlotHalves;
+        for (int kb = 0; kb < L.g.n_kb; ++kb) {
           for (int kx = 0; kx < 3; ++kx, ++a_it) {
             const uint32_t sa = a_it % kPlStages;
             D3B_WAIT(a_empty(sa), ((a_it / kPlStages) & 1u) ^ 1u, 1);
             mbar_arrive_expect_tx(a_full(sa), kPlAStageBytes);
             const uint32_t dst = a_base + sa * kPlAStageBytes;
-            tma_load_4d(dst, tm_hi, kb * kBvKc, x0 + kx - g.pad, y0 - g.pad, b, a_full(sa));
+            tma_load_4d(dst, &L.tm_hi, kb * kBvKc, x0 + kx - L.g.pad, y0 - L.g.pad, b, a_full(sa));
             if constexpr (PLANES == 2)
-              tma_load_4d(dst + kPlPatchBytes, tm_lo, kb * kBvKc, x0 + kx - g.pad, y0 - g.pad, b, a_full(sa));
+              tma_load_4d(dst + kPlPatchBytes, &L.tm_lo, kb * kBvKc, x0 + kx - L.g.pad, y0 - L.g.pad, b, a_full(sa));
             for (int ky = 0; ky < 3; ++ky, ++b_it) {
               const uint32_t sb = b_it % kPlStages;
               D3B_WAIT(b_empty(sb), ((b_it / kPlStages) & 1u) ^ 1u, 2);
               mbar_arrive_expect_tx(b_full(sb), kPlBBytes);
-              tma_bulk_g2s(b_base + sb * kPlBBytes, wgrp + ((size_t)(ky * 3 + kx) * g.n_kb + kb) * kPlSlotHalves,
+              tma_bulk_g2s(b_base + sb * kPlBBytes, wgrp + ((size_t)(ky * 3 + kx) * L.g.n_kb + kb) * kPlSlotHalves,
                            kPlBBytes, b_full(sb));
             }
           }
         }
+        if (!P.work) t += gridDim.x;
       }
     }
   } else {
@@ -388,14 +484,26 @@ __device__ __forceinline__ void bev_conv16_pl_body(const CUtensorMap* tm_hi, con
     const int m = warp >> 2, wq = warp & 3;
     bool ovf = false;
     uint32_t a_it = 0, b_it = 0;                 // ring positions of the tile's first A / B stage
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      int grp, b, y0, x0;
-      decode(tile, grp, b, y0, x0);
+    uint32_t it = 0;                             // tickets taken from the ring
+    auto next_ticket = [&]() {
+      const uint32_t ts = it & 1u;
+      D3B_WAIT(tk_full(ts), (it >> 1) & 1u, 8);
+      const int t = tk_ring[ts];
+      __syncwarp();
+      if (lane == 0) mbar_arrive(tk_empty(ts));
+      ++it;
+      return t;
+    };
+    for (int t = next_ticket(); t < n_tickets;) {
+      int l, grp, b, y0, x0, sp;
+      decode(t, l, grp, b, y0, x0, sp);
+      const PlLayer& L = P.layer[l];
+      const int n_slots = 9 * L.g.n_kb;                                // (kb, kx, ky), ky fastest
       float acc[kPlCout / 2], p0[kPlCout / 2], p1[kPlCout / 2];
 #pragma unroll
       for (int q = 0; q < kPlCout / 2; ++q) acc[q] = 0.f;
       // slot s = (kb, kx, ky): its 12 MMAs into the partial P, committed as one group
-      auto issue = [&](float (&P)[kPlCout / 2], int s) {
+      auto issue = [&](float (&Pp)[kPlCout / 2], int s) {
         const int ky = s % 3;
         const uint32_t ai = a_it + s / 3, bi = b_it + s;
         const uint32_t sa = ai % kPlStages, sb = bi % kPlStages;
@@ -409,20 +517,20 @@ __device__ __forceinline__ void bev_conv16_pl_body(const CUtensorMap* tm_hi, con
           const uint32_t adv = ks * 32;
           if constexpr (PLANES == 2) {
             // small terms first, the dominant hi.hi product last (the order of the pixel-stationary kernel)
-            wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_lo + adv), gmma_desc_sw128(b_hi + adv), ks > 0 ? 1u : 0u);
-            wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_lo + adv), 1u);
-            wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + adv), 1u);
+            wgmma_f16<kPlCout>(Pp, gmma_desc_sw128(a_lo + adv), gmma_desc_sw128(b_hi + adv), ks > 0 ? 1u : 0u);
+            wgmma_f16<kPlCout>(Pp, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_lo + adv), 1u);
+            wgmma_f16<kPlCout>(Pp, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + adv), 1u);
           } else {
-            wgmma_f16<kPlCout>(P, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + adv), ks > 0 ? 1u : 0u);
+            wgmma_f16<kPlCout>(Pp, gmma_desc_sw128(a_hi + adv), gmma_desc_sw128(b_hi + adv), ks > 0 ? 1u : 0u);
           }
         }
         gmma_commit();
       };
       // slot s has completed: fold its partial (round-to-nearest) and release its stages
-      auto retire = [&](float (&P)[kPlCout / 2], int s) {
-        gmma_fence_regs(P);
+      auto retire = [&](float (&Pp)[kPlCout / 2], int s) {
+        gmma_fence_regs(Pp);
 #pragma unroll
-        for (int q = 0; q < kPlCout / 2; ++q) acc[q] += P[q];
+        for (int q = 0; q < kPlCout / 2; ++q) acc[q] += Pp[q];
         __syncwarp();
         if (lane == 0) {
           mbar_arrive(b_empty((b_it + s) % kPlStages));
@@ -449,6 +557,11 @@ __device__ __forceinline__ void bev_conv16_pl_body(const CUtensorMap* tm_hi, con
 
       // epilogue, column block outer: each column pair's parameters are loaded once and used for both rows of the
       // thread (row outer keeps all 16 blocks' parameters live next to the sums and spills)
+      const BvGeom& g = L.g;
+      const Epi16& epi = L.epi;
+      __half* out_hi = L.out_hi;
+      __half* out_lo = L.out_lo;
+      float* out_f32 = L.out_f32;
       const int cg = grp % g.cgroups;
       const int pcol = grp * kPlCout;           // per-group epilogue parameters are laid out group-major
       const int x = x0 + (lane >> 2);
@@ -488,27 +601,46 @@ __device__ __forceinline__ void bev_conv16_pl_body(const CUtensorMap* tm_hi, con
           if (out_f32) *reinterpret_cast<float2*>(out_f32 + row_off[h] + col) = make_float2(v0, v1);
         }
       }
-      // one flag write per thread, after its last tile (placed after the tile loop, it costs 40 registers: ptxas
-      // then spills the sums)
-      if (tile + (int)gridDim.x >= n_tiles && ovf && overflow) atomicOr(overflow, 1);
+      // publish the tile to the next layer of the chain
+      if (P.work && l + 1 < P.n_layers) {
+        fence_proxy_async_global();
+        asm volatile("bar.sync 1, %0;" ::"n"(32 * kBvMathWarps) : "memory");
+        if (threadIdx.x == 0) {
+          __threadfence();
+          red_release_gpu_add(P.work + 2 + (size_t)l * P.spatial + sp, 1u);
+        }
+      }
+      t = next_ticket();
+      // one flag write per thread, once it knows it has no further tile (placed after the tile loop, it costs 40
+      // registers: ptxas then spills the sums)
+      if (t >= n_tickets && ovf && P.overflow) atomicOr(P.overflow, 1);
     }
   }
-  D3B_CTA_MARK(1, epi.seq);
+  if (P.work) {
+    // the last CTA out resets the counters for the next launch (or graph replay)
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      __threadfence();
+      unsigned int prev;
+      asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], 1;" : "=r"(prev) : "l"(P.work + 1) : "memory");
+      last_cta = prev == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (last_cta) {
+      const int n_words = 2 + (P.n_layers - 1) * P.spatial;
+      for (int i = threadIdx.x; i < n_words; i += blockDim.x) P.work[i] = 0u;
+    }
+  }
+  D3B_CTA_MARK(1, P.seq);
 }
 
-__global__ void __launch_bounds__(kBvThreads, 1)
-bev_conv16_pl_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, BvGeom g,
-                     const __half* __restrict__ packed, Epi16 epi, __half* __restrict__ out_hi,
-                     __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
-  bev_conv16_pl_body<2>(&tm_hi, &tm_lo, g, packed, epi, out_hi, out_lo, out_f32, overflow);
+__global__ void __launch_bounds__(kBvThreads, 1) bev_conv16_pl_kernel(const __grid_constant__ PlChain P) {
+  bev_conv16_pl_body<2>(P);
 }
 
 // Single-pass FP16 (tm_lo, out_lo unused).
-__global__ void __launch_bounds__(kBvThreads, 1)
-bev_conv16_pl_f16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, BvGeom g,
-                         const __half* __restrict__ packed, Epi16 epi, __half* __restrict__ out_hi,
-                         __half* __restrict__ out_lo, float* __restrict__ out_f32, int* __restrict__ overflow) {
-  bev_conv16_pl_body<1>(&tm_hi, &tm_lo, g, packed, epi, out_hi, out_lo, out_f32, overflow);
+__global__ void __launch_bounds__(kBvThreads, 1) bev_conv16_pl_f16_kernel(const __grid_constant__ PlChain P) {
+  bev_conv16_pl_body<1>(P);
 }
 
 // ---- host side: tensor maps through the driver entry point (libcuda is not linked: CPU hosts must dlopen us) ----------
@@ -594,30 +726,42 @@ static int launch_bev(const d3b_bev16_params* p, const BvGeom& g, cudaStream_t s
   return D3B_OK;
 }
 
-// pipelined variant: 3x3, stride 1, output blocks of 128 channels, C_in % 64 == 0, no sub-pixel groups
+// pipelined kernel over layers[0, n) (3x3, stride 1, output blocks of 128 channels, C_in % 64 == 0, pad 1, no
+// sub-pixel groups); work = null: one layer, static tile walk
 template <int PLANES>
-static int launch_bev_pl(const d3b_bev16_params* p, BvGeom g, cudaStream_t stream) {
+static int launch_bev_pl(const d3b_bev16_params* layers, const BvGeom* gs, int n, unsigned int* work,
+                         cudaStream_t stream) {
   constexpr auto kernel = PLANES == 2 ? bev_conv16_pl_kernel : bev_conv16_pl_f16_kernel;
   static SmemOptIn optin;
   D3B_CUDA(ensure_dynamic_smem(kernel, PlCfg<PLANES>::kSmemBytes, optin));
-  CUtensorMap tm_hi, tm_lo;
-  Epi16 e;
-  const int st = bev_args(p, PLANES, kBvHalfX, kBvTileY + 2, 1, &tm_hi, &tm_lo, &e);
-  if (st != D3B_OK) return st;
-  g.tiles_x = div_up(g.w_out, kBvHalfX);     // tiles of 16 rows x 8 columns
-  D3B_CUDA(launch_maybe_pdl(kernel, dim3(bev_grid(g)), dim3(kBvThreads), PlCfg<PLANES>::kSmemBytes, stream, tm_hi, tm_lo,
-                            g, (const __half*)p->weight_packed, e, (__half*)p->out_hi, (__half*)p->out_lo, p->out_f32,
-                            (int*)p->overflow));
+  PlChain c = {};
+  c.n_layers = n;
+  for (int k = 0; k < n; ++k) {
+    const d3b_bev16_params* p = layers + k;
+    PlLayer& L = c.layer[k];
+    const int st = bev_args(p, PLANES, kBvHalfX, kBvTileY + 2, 1, &L.tm_hi, &L.tm_lo, &L.epi);
+    if (st != D3B_OK) return st;
+    L.g = gs[k];
+    L.g.tiles_x = div_up(L.g.w_out, kBvHalfX);     // tiles of 16 rows x 8 columns
+    L.packed = (const __half*)p->weight_packed;
+    L.out_hi = (__half*)p->out_hi;
+    L.out_lo = (__half*)p->out_lo;
+    L.out_f32 = p->out_f32;
+    c.spatial = L.g.batch * L.g.tiles_y * L.g.tiles_x;
+    c.first_ticket[k + 1] = c.first_ticket[k] + c.spatial * L.g.groups;
+  }
+  c.seq = c.layer[0].epi.seq;
+  c.overflow = (int*)layers[0].overflow;
+  c.work = work;
+  const int n_tickets = c.first_ticket[n];
+  D3B_CUDA(launch_maybe_pdl(kernel, dim3(n_tickets < kNumSMs ? n_tickets : kNumSMs), dim3(kBvThreads),
+                            PlCfg<PLANES>::kSmemBytes, stream, c));
   D3B_LAUNCH_CHECK();
   return D3B_OK;
 }
 
-}  // namespace d3b
-
-using namespace d3b;
-
-extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
+// The argument checks of d3b_bev_conv16 (before any CUDA call); fills the conv geometry and the plane count.
+static int bev_check(const d3b_bev16_params* p, BvGeom* gp, bool* two_planes) {
   D3B_REQUIRE(p && p->in_hi && p->weight_packed, "d3b_bev_conv16: null argument");
   PlanePairs pp;
   pp.add(p->in_hi, p->in_lo);
@@ -625,7 +769,7 @@ extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
   D3B_REQUIRE(pp.consistent(),
               "d3b_bev_conv16: give in_lo and out_lo with their hi planes (FP16x3) or neither (single-pass FP16); got "
               "in_lo %s, out_lo %s", p->in_lo ? "set" : "NULL", p->out_lo ? "set" : "NULL");
-  const bool two = pp.planes() == 2;
+  *two_planes = pp.planes() == 2;
   D3B_REQUIRE(p->batch >= 1 && p->h_in >= 1 && p->w_in >= 1 && p->c_in >= 16 && p->c_in % 16 == 0,
               "d3b_bev_conv16: bad input shape [%d,%d,%d,%d] (C_in must be a multiple of 16)", p->batch, p->h_in, p->w_in, p->c_in);
   // kernel = stride = s (2..4): the strided Conv2d deblock; it tiles the input exactly, so it takes no padding
@@ -645,7 +789,7 @@ extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
   // (an input smaller than the kernel has no output; C division would round -1/s up to 0 and make one)
   D3B_REQUIRE(p->h_in + 2 * p->pad >= p->ksize && p->w_in + 2 * p->pad >= p->ksize,
               "d3b_bev_conv16: input %dx%d (pad %d) is smaller than the kernel %d", p->h_in, p->w_in, p->pad, p->ksize);
-  BvGeom g;
+  BvGeom& g = *gp;
   g.batch = p->batch;
   g.h_out = (p->h_in + 2 * p->pad - p->ksize) / p->stride + 1;
   g.w_out = (p->w_in + 2 * p->pad - p->ksize) / p->stride + 1;
@@ -658,11 +802,29 @@ extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
   g.groups = p->groups; g.cgroups = p->cgroups; g.up = p->up;
   g.out_h = g.h_out * p->up; g.out_w = g.w_out * p->up;
   g.out_channels = p->out_channels; g.out_c0 = p->out_c0;
+  return D3B_OK;
+}
+
+// the layers the pipelined kernel takes: 3x3 stride 1, output blocks of 128 channels, C_in % 64 == 0, no sub-pixel groups
+static bool pl_eligible(const d3b_bev16_params* p) {
+  return p->ksize == 3 && p->stride == 1 && p->c_out == kPlCout && p->c_in % kBvKc == 0 && p->up == 1;
+}
+
+}  // namespace d3b
+
+using namespace d3b;
+
+extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  BvGeom g;
+  bool two;
+  const int st = bev_check(p, &g, &two);
+  if (st != D3B_OK) return st;
   // Automatic (variant 2) = the pipelined kernel for the 3x3 stride-1 layers with 128-channel output blocks, the
   // pixel-stationary kernel for every other shape.  Variant 0 (pixel-stationary everywhere) is the reference the
   // pipelined kernel reproduces bit for bit.
-  const bool s1_blocks = p->ksize == 3 && p->stride == 1 && p->c_out == kPlCout && p->c_in % kBvKc == 0 && p->up == 1;
-  if (bev_variant() == 2 && s1_blocks) return two ? launch_bev_pl<2>(p, g, stream) : launch_bev_pl<1>(p, g, stream);
+  if (bev_variant() == 2 && pl_eligible(p))
+    return two ? launch_bev_pl<2>(p, &g, 1, nullptr, stream) : launch_bev_pl<1>(p, &g, 1, nullptr, stream);
 #define D3B_BEV_CASE(KS, ST)                                                                                        \
   if (p->ksize == KS && p->stride == ST) {                                                                          \
     switch (p->c_out) {                                                                                             \
@@ -681,6 +843,58 @@ extern "C" int d3b_bev_conv16(const d3b_bev16_params* p, void* stream_) {
 #undef D3B_BEV_CASE
   set_error("d3b_bev_conv16: C_out per group %d not in {32, 64, 128}", p->c_out);
   return D3B_ERR_UNSUPPORTED;
+}
+
+extern "C" int64_t d3b_bev_conv16_chain_workspace_bytes(int32_t batch, int32_t h, int32_t w, int32_t n_layers) {
+  if (batch < 1 || h < 1 || w < 1 || n_layers < 1 || n_layers > kPlMaxLayers) return 0;
+  const int64_t tiles = (int64_t)batch * div_up(h, kBvTileY) * div_up(w, kBvHalfX);
+  return 4 * (2 + (int64_t)(n_layers - 1) * tiles);     // ticket and exit counters, done counters of layers 0..n-2
+}
+
+extern "C" int d3b_bev_conv16_chain(const d3b_bev16_params* layers, int32_t n_layers, void* workspace,
+                                    int64_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  D3B_REQUIRE(layers && n_layers >= 1 && n_layers <= kPlMaxLayers, "d3b_bev_conv16_chain: n_layers %d outside 1..%d",
+              n_layers, kPlMaxLayers);
+  BvGeom gs[kPlMaxLayers];
+  bool two = false;
+  for (int k = 0; k < n_layers; ++k) {
+    const d3b_bev16_params* p = layers + k;
+    bool tk;
+    if (bev_check(p, &gs[k], &tk) != D3B_OK) {
+      char why[256];
+      snprintf(why, sizeof(why), "%s", d3b_last_error());
+      set_error("d3b_bev_conv16_chain: layer %d: %s", k, why);
+      return D3B_ERR_INVALID_ARG;
+    }
+    D3B_REQUIRE(pl_eligible(p) && p->pad == 1 && p->out_hi && p->out_c0 == 0 && p->out_channels == p->cgroups * p->c_out,
+                "d3b_bev_conv16_chain: layer %d is not a 3x3 stride-1 pad-1 layer of 128-channel output blocks with "
+                "C_in %% 64 == 0 writing whole output planes", k);
+    D3B_REQUIRE(p->in_hi != p->out_hi && (p->in_lo == nullptr || p->in_lo != p->out_lo),
+                "d3b_bev_conv16_chain: layer %d's input aliases its own output", k);
+    if (k == 0) {
+      two = tk;
+      continue;
+    }
+    const d3b_bev16_params* q = layers + k - 1;
+    D3B_REQUIRE(tk == two && p->batch == q->batch && p->h_in == q->h_in && p->w_in == q->w_in &&
+                    p->c_in == q->out_channels && p->in_hi == q->out_hi && p->in_lo == q->out_lo,
+                "d3b_bev_conv16_chain: layer %d's input is not layer %d's output planes", k, k - 1);
+    D3B_REQUIRE(p->overflow == layers[0].overflow, "d3b_bev_conv16_chain: layer %d has another overflow flag than layer 0",
+                k);
+  }
+  const int64_t need = d3b_bev_conv16_chain_workspace_bytes(layers[0].batch, layers[0].h_in, layers[0].w_in, n_layers);
+  D3B_REQUIRE(workspace && workspace_bytes >= need, "d3b_bev_conv16_chain: workspace of %lld bytes, %lld needed",
+              (long long)workspace_bytes, (long long)need);
+  if (bev_variant() != 2) {             // the reference schedule: layer by layer through d3b_bev_conv16
+    for (int k = 0; k < n_layers; ++k) {
+      const int st = d3b_bev_conv16(layers + k, stream_);
+      if (st != D3B_OK) return st;
+    }
+    return D3B_OK;
+  }
+  unsigned int* work = (unsigned int*)workspace;
+  return two ? launch_bev_pl<2>(layers, gs, n_layers, work, stream) : launch_bev_pl<1>(layers, gs, n_layers, work, stream);
 }
 
 #ifdef D3B_SOFT_TIMEOUT

@@ -259,7 +259,8 @@ def rpn_is_fusable16(rpn):
 
 class FusedBevStack:
     """RPN + all task heads on NHWC f16 planes (FP16x3, or single-pass FP16 when the input carries one plane: every
-    layer then runs on one plane, with the same packed weights): one launch per conv layer, the deblocks write straight into
+    layer then runs on one plane, with the same packed weights): one launch per conv layer, except that each block's run
+    of 3x3 stride-1 layers is one chained launch (conv16.bev_chain), the deblocks write straight into
     their channel slice of the concat buffer, and the heads of all tasks are ONE 1x1 conv whose fp32 output rows are
     already the NHWC-permuted layout `Head.forward` produces (mg_head.py:214-230)."""
 
@@ -318,6 +319,14 @@ class FusedBevStack:
             p = self._bufs[key] = conv16.Planes(shape, device, n_planes=n_planes)
         return p
 
+    def _chain_workspace(self, b, h, w, n, device):
+        # owned by the stack and keyed by shape, so a captured graph bakes in a pointer that stays valid
+        key = ("chain", b, h, w, n)
+        ws = self._bufs.get(key)
+        if ws is None:
+            ws = self._bufs[key] = conv16.chain_workspace(b, h, w, n, device)
+        return ws
+
     def layers(self):
         """Flat (tag, layer) list in execution order (bench / accounting)."""
         out = []
@@ -342,11 +351,23 @@ class FusedBevStack:
             concat = None
             col = 0
             for i, blk in enumerate(pl["blocks"]):
-                for j, layer in enumerate(blk):
-                    ho, wo = layer.out_hw(x.shape[1], x.shape[2])
-                    out = self._planes(("blk", i, j % 2), (b, ho, wo, layer.c_out_padded), device, n_planes)
-                    layer(x, out=out, overflow=overflow, tag="bev3x3" if layer.ksize == 3 else "bev1x1")
-                    x = out
+                j = 0
+                while j < len(blk):
+                    # a run of consecutive 3x3 stride-1 layers is one chained launch (at most 8 layers each)
+                    n = 1
+                    while blk[j].chainable and n < 8 and j + n < len(blk) and blk[j + n].chainable:
+                        n += 1
+                    ho, wo = blk[j].out_hw(x.shape[1], x.shape[2])
+                    outs = [self._planes(("blk", i, (j + k) % 2), (b, ho, wo, blk[j + k].c_out_padded), device, n_planes)
+                            for k in range(n)]
+                    if n == 1:
+                        layer = blk[j]
+                        layer(x, out=outs[0], overflow=overflow, tag="bev3x3" if layer.ksize == 3 else "bev1x1")
+                    else:
+                        conv16.bev_chain(blk[j:j + n], x, outs, self._chain_workspace(b, ho, wo, n, device),
+                                         overflow=overflow)
+                    x = outs[-1]
+                    j += n
                 k = i - pl["start"]
                 if k >= 0:
                     de = pl["deblocks"][k]

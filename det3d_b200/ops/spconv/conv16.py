@@ -238,9 +238,29 @@ class BevConv16:
         wo = (w + 2 * self.pad - self.ksize) // self.stride + 1
         return ho * self.up, wo * self.up
 
+    @property
+    def chainable(self):
+        """True for the layers d3b_bev_conv16_chain takes: 3x3, stride 1, pad 1, output blocks of 128 channels,
+        C_in a multiple of 64."""
+        return (self.ksize == 3 and self.stride == 1 and self.pad == 1 and self.up == 1 and self.c_blk == 128
+                and self.c_in % 64 == 0)
+
     def __call__(self, x, out=None, out_f32=None, out_c0=0, overflow=None, tag="bev"):
         """x: Planes [B, H, W, C_in]; out: Planes [B, H', W', C_total] (as many planes as x) and/or out_f32
         [B, H', W', C_total] fp32.  One input plane runs the single-pass FP16 kernels."""
+        b, h, w = x.shape[:3]
+        p = self.params(x, out, out_f32, out_c0, overflow)
+        ho, wo = self.out_hw(h, w)
+        with _lib.on_device_of(x.buf), _lib.timed(tag, flops=self.flops(b, h, w), c_in=self.c_in, c_out=self.c_out_total,
+                                                  ksize=self.ksize, stride=self.stride, up=self.up, math=math_of(x),
+                                                  pixels_in=b * h * w, pixels_out=b * ho * wo,
+                                                  tiles=b * (-(-(ho // self.up) // 16)) * (-(-(wo // self.up) // 16)) * self.groups):
+            st = _lib.lib().d3b_bev_conv16(C.byref(p), _lib.current_stream())
+        _lib.check(st, "d3b_bev_conv16")
+        return out if out is not None else out_f32
+
+    def params(self, x, out=None, out_f32=None, out_c0=0, overflow=None):
+        """The d3b_bev16_params of one call (see __call__)."""
         b, h, w, c = x.shape
         assert c == self.c_in
         p = Bev16Params()
@@ -270,16 +290,40 @@ class BevConv16:
                 assert tuple(out_f32.shape) == tuple(out.shape)
             p.out_f32 = out_f32.data_ptr()
         p.overflow = _lib.ptr(overflow)
-        with _lib.on_device_of(x.buf), _lib.timed(tag, flops=self.flops(b, h, w), c_in=self.c_in, c_out=self.c_out_total,
-                                                  ksize=self.ksize, stride=self.stride, up=self.up, math=math_of(x),
-                                                  pixels_in=b * h * w, pixels_out=b * ho * wo,
-                                                  tiles=b * (-(-(ho // self.up) // 16)) * (-(-(wo // self.up) // 16)) * self.groups):
-            st = _lib.lib().d3b_bev_conv16(C.byref(p), _lib.current_stream())
-        _lib.check(st, "d3b_bev_conv16")
-        return out if out is not None else out_f32
+        return p
 
     def flops(self, b, h, w):
         """fp32-equivalent flops of one call on a [b, h, w] input grid."""
         ho = (h + 2 * self.pad - self.ksize) // self.stride + 1
         wo = (w + 2 * self.pad - self.ksize) // self.stride + 1
         return 2 * b * ho * wo * self.ksize * self.ksize * self.c_in * self.c_out_total * self.up * self.up
+
+
+def chain_workspace(batch, h, w, n_layers, device):
+    """A zeroed workspace for d3b_bev_conv16_chain over n_layers layers of a [batch, h, w] grid (every call leaves it
+    zero again)."""
+    n = int(_lib.lib().d3b_bev_conv16_chain_workspace_bytes(batch, h, w, n_layers))
+    if n == 0:
+        raise _lib.D3BError("d3b_bev_conv16_chain: no workspace for %d layers over %dx%dx%d" % (n_layers, batch, h, w))
+    return torch.zeros((n + 3) // 4, dtype=torch.int32, device=device)
+
+
+def bev_chain(layers, x, outs, workspace, overflow=None, tag="bev3x3"):
+    """Runs `layers` (each `chainable`) as ONE launch of d3b_bev_conv16_chain: layer k reads outs[k - 1] (x for k = 0)
+    and writes outs[k] (Planes of the same grid).  Bit-identical to calling the layers one by one."""
+    n = len(layers)
+    assert n == len(outs) and all(l.chainable for l in layers)
+    arr = (Bev16Params * n)()
+    src, flops = x, 0
+    for k, (layer, out) in enumerate(zip(layers, outs)):
+        arr[k] = layer.params(src, out=out, overflow=overflow)
+        flops += layer.flops(*src.shape[:3])
+        src = out
+    b, h, w, c = x.shape
+    # one launch: `flops` is the chain's total, the rest describes its first layer
+    with _lib.on_device_of(x.buf), _lib.timed(tag, flops=flops, layers=n, c_in=c, c_out=layers[0].c_out_total, ksize=3,
+                                              stride=1, up=1, math=math_of(x), pixels_in=b * h * w, pixels_out=b * h * w):
+        st = _lib.lib().d3b_bev_conv16_chain(arr, n, workspace.data_ptr(), workspace.numel() * workspace.element_size(),
+                                             _lib.current_stream())
+    _lib.check(st, "d3b_bev_conv16_chain")
+    return outs[-1]

@@ -394,6 +394,21 @@ typedef struct {
 
 int d3b_bev_conv16(const d3b_bev16_params* p, void* stream);
 
+/* A chain of n_layers (1..8) 3x3 stride-1 layers over one grid, run as ONE persistent launch that hands out the tiles
+ * of every layer in order: a tile of layer k starts as soon as the <= 9 tiles of layer k - 1 it reads are written,
+ * so the tail of one layer overlaps the head of the next.  Every layer must be one d3b_bev_conv16 would run on the
+ * pipelined kernel (ksize 3, stride 1, pad 1, c_out 128 per group, c_in % 64 == 0, up 1) and write whole output planes
+ * (out_hi set, out_c0 0, out_channels = cgroups * 128); layer k's in_hi / in_lo must be layer k - 1's out_hi / out_lo,
+ * no layer may write its own input, and all layers share layer 0's overflow flag.  Layer k may write the planes layer
+ * k - 1 read (the ping-pong of an RPN block).  `workspace` holds the launch's tile counters: at least
+ * d3b_bev_conv16_chain_workspace_bytes(batch, h_in, w_in, n_layers) bytes, zero before the first call; every call
+ * leaves it zero again, so a captured graph replays with no host action.  Results are bit-identical to the layers run
+ * one by one.  Under d3b_set_bev_variant(0) the layers run one by one through d3b_bev_conv16.  Argument errors
+ * return D3B_ERR_INVALID_ARG before any CUDA call. */
+int64_t d3b_bev_conv16_chain_workspace_bytes(int32_t batch, int32_t h, int32_t w, int32_t n_layers);
+int d3b_bev_conv16_chain(const d3b_bev16_params* layers, int32_t n_layers, void* workspace, int64_t workspace_bytes,
+                         void* stream);
+
 /* ========================================================================= *
  * 4. Rotated-box BEV IoU / NMS
  * ========================================================================= */
