@@ -25,6 +25,7 @@ from det3d_b200.datasets.pipelines.loading import (MAX_BATCH, MAX_SWEEPS, Batche
                                                     sweep_table_capacity)
 from det3d_b200.models import build_detector
 from det3d_b200.ops.point_cloud.frustum import MAX_NDIM, MIN_NDIM, FrustumCrop
+from det3d_b200.ops.point_cloud.kitti_results import KittiResults, calib_table, check_calibs, to_annos
 from det3d_b200.ops.point_cloud.voxelize import Voxelizer
 
 
@@ -54,12 +55,13 @@ class InferencePipeline:
         self.strict_fp32 = strict_fp32
         # (batch, bucket, ndim) -> _GraphEntry, (batch, raw bucket, table capacity, raw_stride, n_feat) ->
         # _SweepGraphEntry (infer_sweeps) and ("stream", B, K, slot_capacity, raw_stride, n_feat) -> _StreamGraphEntry
-        # (SweepStream.infer) and ("frustum", B, raw bucket, ndim) -> _FrustumGraphEntry (infer_raw), least recently
-        # used first
+        # (SweepStream.infer) and ("frustum", B, raw bucket, ndim) / ("frustum_kitti", B, raw bucket, ndim) ->
+        # _FrustumGraphEntry (infer_raw without / with kitti_results), least recently used first
         self._graphs = collections.OrderedDict()
         self.max_graphs = 8
         self._ovf_host = None
         self._planes = collections.OrderedDict()      # calibration bytes -> frustum planes f64 [6, 4] (infer_raw)
+        self._kitti_tables = collections.OrderedDict()   # calibration bytes -> KITTI results table f64 [32]
 
     def anchors(self, batch):
         a = self._anchor_cache.get(batch)
@@ -241,13 +243,18 @@ class InferencePipeline:
         if pinned_out is None:
             pinned_out = torch.empty(packed.shape, dtype=torch.float32, pin_memory=True)
         pinned_out.copy_(packed, non_blocking=True)
+        return pinned_out, self._sync_overflow()
+
+    def _sync_overflow(self):
+        """D2H of the f16-range flag behind the copies already enqueued, then one sync.  Returns True when the flag was
+        raised and the model has switched to tf32x3 (check_overflow)."""
         flag = self.overflow_flag()
         if flag is not None:
             if self._ovf_host is None:
                 self._ovf_host = torch.zeros(1, dtype=torch.int32, pin_memory=True)
             self._ovf_host.copy_(flag, non_blocking=True)
         torch.cuda.current_stream().synchronize()
-        return pinned_out, flag is not None and self.check_overflow(int(self._ovf_host[0]))
+        return flag is not None and self.check_overflow(int(self._ovf_host[0]))
 
     @torch.no_grad()
     def infer_sweeps(self, samples, pinned_out=None, graphed=False, n_feat=4, radius=1.0):
@@ -326,38 +333,44 @@ class InferencePipeline:
             raise ValueError("raw clouds must have %d to %d columns, got %d" % (MIN_NDIM, MAX_NDIM, ndim))
         if sum(sizes) > 1 << 30:
             raise ValueError("more than 2^30 raw points in one batch")
-        for b, cal in enumerate(calibs):
-            if not isinstance(cal, dict) or not all(k in cal for k in ("rect", "Trv2c", "P2", "image_shape")):
-                raise ValueError("calibration %d: expected dict(rect, Trv2c, P2, image_shape)" % b)
-            if np.shape(cal["rect"]) != (4, 4) or np.shape(cal["Trv2c"]) != (4, 4):
-                raise ValueError("calibration %d: rect and Trv2c must be 4x4 (the info files' extended form)" % b)
-            if np.shape(cal["P2"]) not in ((3, 4), (4, 4)):
-                raise ValueError("calibration %d: P2 must be 3x4 or 4x4, got shape %s" % (b, np.shape(cal["P2"])))
-            shape = np.asarray(cal["image_shape"]).reshape(-1)
-            if shape.shape[0] < 2 or not np.all(shape[:2] > 0):
-                raise ValueError("calibration %d: image_shape must be (H, W) > 0, got %r" % (b, cal["image_shape"]))
+        check_calibs(calibs)
         return ndim, sizes
 
-    def frustum_planes(self, calib):
-        """camera_frustum_planes of one calibration, cached by the calibration's bytes (KITTI calibrations change per
-        drive, not per frame)."""
-        # keyed on each matrix's dtype, shape and bytes: the planes are computed from the arrays as given, and numpy's
+    @staticmethod
+    def _cached_per_calib(cache, calib, compute):
+        """compute(calib, (H, W)) cached by the calibration's bytes (KITTI calibrations change per drive, not per
+        frame), the 256 most recently used kept."""
+        # keyed on each matrix's dtype, shape and bytes: the tables are computed from the arrays as given, and numpy's
         # inv / qr give a float32 calibration other planes than the same values in float64
         parts = [np.ascontiguousarray(calib[k]) for k in ("rect", "Trv2c", "P2")]
         shape = tuple(int(v) for v in np.asarray(calib["image_shape"]).reshape(-1)[:2])
         key = b"".join(p.tobytes() for p in parts) + repr((shape, [(p.dtype.str, p.shape) for p in parts])).encode()
-        planes = self._planes.get(key)
-        if planes is None:
-            planes = camera_frustum_planes(calib["rect"], calib["Trv2c"], calib["P2"], shape)
-            self._planes[key] = planes
-            while len(self._planes) > 256:
-                self._planes.popitem(last=False)
+        value = cache.get(key)
+        if value is None:
+            value = cache[key] = compute(calib, shape)
+            while len(cache) > 256:
+                cache.popitem(last=False)
         else:
-            self._planes.move_to_end(key)
-        return planes
+            cache.move_to_end(key)
+        return value
+
+    def frustum_planes(self, calib):
+        """camera_frustum_planes of one calibration, cached by the calibration's bytes."""
+        return self._cached_per_calib(self._planes, calib, lambda c, shape: camera_frustum_planes(
+            c["rect"], c["Trv2c"], c["P2"], shape))
+
+    def kitti_calib_table(self, calib):
+        """The KITTI results kernel's calibration row f64 [32] (ops.point_cloud.kitti_results.calib_table: rect @ Trv2c
+        by numpy's matmul, P2, the image shape), cached by the calibration's bytes."""
+        return self._cached_per_calib(self._kitti_tables, calib,
+                                      lambda c, shape: calib_table(dict(c, image_shape=shape)))
+
+    def class_names(self):
+        """The config's class names flattened over its tasks, the order predict's labels index."""
+        return [n for t in self.cfg.tasks for n in t["class_names"]]
 
     @torch.no_grad()
-    def infer_raw(self, clouds, calibs, pinned_out=None, graphed=False):
+    def infer_raw(self, clouds, calibs, pinned_out=None, graphed=False, kitti_results=False):
         """Raw KITTI scans -> host detections [B, D, nd+3], as infer_host: each scan is first cropped to its camera's
         view frustum (box_np_ops.remove_outside_points, bit-exact), on the device.
 
@@ -369,10 +382,20 @@ class InferencePipeline:
         raw bucket, ndim) (bucket_of of the raw total), in the LRU of forward_graphed; the scans are copied into its
         static raw buffer, and the offsets and the plane table H2D only when they differ from that graph's last
         replay.  The voxelizer's capacity is the raw bucket (the crop only removes points).  Raises ValueError before
-        anything is enqueued when the arguments are malformed.  The overflow fallback is infer_host's."""
+        anything is enqueued when the arguments are malformed.  The overflow fallback is infer_host's.
+
+        kitti_results=True returns instead what the reference reports for KITTI
+        (KittiDataset.convert_detection_to_kitti_annos, det3d/datasets/kitti/kitti.py:78-158): one anno dict per scan
+        with the reference's keys and dtypes, holding the detections whose image box meets the image, in predict's
+        order -- their clipped image box, alpha, camera-frame dimensions, location and rotation_y, score and class
+        name (self.class_names()).  d3b_kitti_results_dev runs right after predict, inside the same graph when
+        graphed (keyed ("frustum_kitti", B, raw bucket, ndim), apart from the plain one); each scan's calibration table
+        (kitti_calib_table, cached per calibration) goes H2D only when it differs from that graph's last replay, and
+        the kept rows, their counts and the f16-range flag come back in one D2H before one sync."""
         clouds, calibs = list(clouds), list(calibs)
         ndim, sizes = self.check_raw_clouds(clouds, calibs)
         planes = np.stack([self.frustum_planes(c) for c in calibs])
+        tables = np.stack([self.kitti_calib_table(c) for c in calibs]) if kitti_results else None
         offsets = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int32)
         batch, bucket = len(clouds), self.bucket_of(int(offsets[-1]))
         if not graphed:
@@ -380,29 +403,47 @@ class InferencePipeline:
             _stage_clouds(clouds, offsets, crop.points)
             crop.set_table(offsets, planes)
             points, cloud_offsets = crop.launch()
+            if kitti_results:
+                kitti = KittiResults(batch, self.device)
+                kitti.set_calib(tables)
         for _attempt in range(2):
             if graphed:         # (a re-run after an overflow captures a new graph: check_overflow dropped them all)
-                entry = self._frustum_graph_entry(batch, bucket, ndim)
-                entry.stage(clouds, offsets, planes)
-                crop = entry.crop
-                packed = self._run_graph(entry, lambda: self.pack(self.forward_device(*crop.launch())))
+                entry = self._frustum_graph_entry(batch, bucket, ndim, kitti_results)
+                entry.stage(clouds, offsets, planes, tables)
+                crop, kitti = entry.crop, entry.kitti
+                if kitti_results:
+                    step = lambda: kitti.launch(self.pack(self.forward_device(*crop.launch())))   # noqa: E731
+                else:
+                    step = lambda: self.pack(self.forward_device(*crop.launch()))                 # noqa: E731
+                out = self._run_graph(entry, step)
             else:
-                packed = self.pack(self.forward_device(points, cloud_offsets))
-            pinned_out, rerun = self._fetch(packed, pinned_out)
+                out = self.pack(self.forward_device(points, cloud_offsets))
+                if kitti_results:
+                    out = kitti.launch(out)
+            if kitti_results:
+                kitti.results_host.copy_(out[0], non_blocking=True)
+                kitti.counts_host.copy_(out[1], non_blocking=True)
+                rerun = self._sync_overflow()
+            else:
+                pinned_out, rerun = self._fetch(out, pinned_out)
             if not rerun:
                 break
+        if kitti_results:
+            return to_annos(kitti.results_host.numpy(), kitti.counts_host.numpy(), self.class_names())
         return pinned_out
 
-    def _frustum_graph_entry(self, batch, bucket, ndim):
-        """The infer_raw graph of ("frustum", batch, bucket, ndim), in the LRU of forward_graphed."""
-        key = ("frustum", batch, bucket, ndim)
+    def _frustum_graph_entry(self, batch, bucket, ndim, kitti_results=False):
+        """The infer_raw graph of ("frustum", batch, bucket, ndim) (kitti_results: ("frustum_kitti", ...), whose entry
+        also holds a KittiResults), in the LRU of forward_graphed."""
+        key = ("frustum_kitti" if kitti_results else "frustum", batch, bucket, ndim)
         entry = self._graphs.get(key)
         if entry is not None:
             self._graphs.move_to_end(key)
             return entry
         while len(self._graphs) >= self.max_graphs:
             self._graphs.popitem(last=False)
-        entry = self._graphs[key] = _FrustumGraphEntry(FrustumCrop(batch, bucket, ndim, self.device))
+        kitti = KittiResults(batch, self.device) if kitti_results else None
+        entry = self._graphs[key] = _FrustumGraphEntry(FrustumCrop(batch, bucket, ndim, self.device), kitti)
         return entry
 
     @staticmethod
@@ -475,23 +516,27 @@ def _stage_clouds(clouds, offsets, points_dev, staging=None):
 
 class _FrustumGraphEntry:
     """Static buffers of one captured infer_raw forward: the FrustumCrop (raw scans, offsets, planes, cropped clouds,
-    their offsets), the pinned staging of the offsets, of the planes and of scans that are not pinned already, the
-    graph and its output."""
+    their offsets), with kitti_results the KittiResults (calibration table, result rows, counts), the pinned staging of
+    the offsets, of the planes, of the calibration table and of scans that are not pinned already, the graph and its
+    output."""
 
-    def __init__(self, crop):
-        self.crop = crop
+    def __init__(self, crop, kitti=None):
+        self.crop, self.kitti = crop, kitti
         self.offsets_staging = torch.zeros(crop.offsets.shape, dtype=torch.int32, pin_memory=True)
         self.planes_staging = torch.zeros(crop.planes.shape, dtype=torch.float64, pin_memory=True)
+        self.calib_staging = None if kitti is None else torch.zeros(kitti.calib.shape, dtype=torch.float64,
+                                                                     pin_memory=True)
         self.raw_staging = None
         self.copied = torch.cuda.Event()
-        self.last_offsets = self.last_planes = None
+        self.last_offsets = self.last_planes = self.last_calib = None
         self.planes_uploads = 0                   # plane-table H2D copies so far
+        self.calib_uploads = 0                    # KITTI calibration-table H2D copies so far
         self.graph = None
         self.out = None
 
-    def stage(self, clouds, offsets, planes):
-        """Enqueue the H2D copies of the scans and, when they differ from the previous replay's, of the offsets and of
-        the plane table."""
+    def stage(self, clouds, offsets, planes, calib_table=None):
+        """Enqueue the H2D copies of the scans and, when they differ from the previous replay's, of the offsets, of
+        the plane table and of the KITTI calibration table."""
         # the pinned staging buffers may still feed the previous copies: wait for those before rewriting them
         self.copied.synchronize()
         crop = self.crop
@@ -504,6 +549,12 @@ class _FrustumGraphEntry:
             crop.planes.copy_(self.planes_staging, non_blocking=True)
             self.last_planes = planes.copy()
             self.planes_uploads += 1
+        if self.kitti is not None and (self.last_calib is None or not np.array_equal(
+                calib_table.view(np.uint64), self.last_calib.view(np.uint64))):
+            self.calib_staging.numpy()[:] = calib_table
+            self.kitti.calib.copy_(self.calib_staging, non_blocking=True)
+            self.last_calib = calib_table.copy()
+            self.calib_uploads += 1
         self.raw_staging = _stage_clouds(clouds, offsets, crop.points, self.raw_staging)
         self.copied.record()
 

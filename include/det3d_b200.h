@@ -176,6 +176,23 @@ int d3b_frustum_crop_dev(const float* points, int32_t point_capacity, int32_t nd
                          const double* planes, int32_t batch, float* out, int32_t* cloud_offsets_out, int32_t* status,
                          void* workspace, size_t workspace_bytes, void* stream);
 
+/* KITTI result rows from predict's packed detections, for graph replay.  replaces the per-box loop of
+ * KittiDataset.convert_detection_to_kitti_annos (det3d/datasets/kitti/kitti.py:78-158): limit_period and the z shift in
+ * f32, box_lidar_to_camera, center_to_corner_box3d (origin (0.5, 1, 0.5), axis 1) and project_to_image (with its column
+ * of ZEROS, so P2's translation never enters) in f64, the strict in-image test, the clip, alpha.
+ * 1 <= batch <= 64, 0 <= max_det <= 2^20, nd 7 or 9 (D3B_ERR_UNSUPPORTED otherwise).
+ * detections [batch][max_det][nd + 3] f32 device: box, score, label, valid (a row counts when valid > 0.5)
+ * calib      [batch][32] f64 DEVICE: M = rect @ Trv2c row-major [0, 16), P2 rows 0..2 row-major [16, 28), image
+ *            height [28] and width [29]; [30, 32) unused
+ * results    [batch][max_det][14] f64 device: per kept detection, in predict's order, bbox (x0, y0, x1, y1) clipped,
+ *            alpha, dimensions (l, h, w), location (camera frame, bottom centre), rotation_y, score, label; rows at or
+ *            past counts[b] are written as zeros
+ * counts     [batch] i32 device: kept detections of each sample
+ * Every f64 product, sum and quotient is rounded on its own in a fixed order (no FMA contraction); sin / cos / atan2 are
+ * the CUDA math library's.  One kernel, one CTA per sample, no host sync, no workspace. */
+int d3b_kitti_results_dev(const float* detections, const double* calib, int32_t batch, int32_t max_det, int32_t nd,
+                          double* results, int32_t* counts, void* stream);
+
 /* ========================================================================= *
  * 2. Rulebook (sparse-convolution index maps)
  *    replaces spconv v1.x `get_indice_pairs` as called by SubMConv3d /
