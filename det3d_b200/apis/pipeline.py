@@ -20,9 +20,8 @@ import torch
 from det3d_b200 import _lib
 from det3d_b200.core.anchor.anchor_generator import anchors_for_tasks
 from det3d_b200.core.bbox.box_np_ops import camera_frustum_planes
-from det3d_b200.datasets.pipelines.loading import (MAX_BATCH, MAX_SWEEPS, BatchedIngest, SweepHistory,
-                                                    check_sweep_samples, ingest_sweeps_batched, stage_raw_sweeps,
-                                                    sweep_table_capacity)
+from det3d_b200.datasets.pipelines.loading import (MAX_BATCH, MAX_SWEEPS, BatchedIngest, RowStager, SweepHistory,
+                                                    check_sweep_samples, sweep_table_capacity)
 from det3d_b200.models import build_detector
 from det3d_b200.ops.point_cloud.frustum import MAX_NDIM, MIN_NDIM, FrustumCrop
 from det3d_b200.ops.point_cloud.kitti_results import KittiResults, calib_table, check_calibs, to_annos
@@ -53,10 +52,10 @@ class InferencePipeline:
         self._anchors = [torch.from_numpy(a).to(self.device) for a in anchors]
         self._anchor_cache = {}
         self.strict_fp32 = strict_fp32
-        # (batch, bucket, ndim) -> _GraphEntry, (batch, raw bucket, table capacity, raw_stride, n_feat) ->
-        # _SweepGraphEntry (infer_sweeps) and ("stream", B, K, slot_capacity, raw_stride, n_feat) -> _StreamGraphEntry
-        # (SweepStream.infer) and ("frustum", B, raw bucket, ndim) / ("frustum_kitti", B, raw bucket, ndim) ->
-        # _FrustumGraphEntry (infer_raw without / with kitti_results), least recently used first
+        # _GraphEntry by key, least recently used first: (batch, bucket, ndim) (forward_graphed, infer_host), (batch,
+        # raw bucket, table capacity, raw_stride, n_feat) (infer_sweeps), ("stream", B, K, slot_capacity, raw_stride,
+        # n_feat) (SweepStream.infer), ("frustum", B, raw bucket, ndim) / ("frustum_kitti", B, raw bucket, ndim)
+        # (infer_raw without / with kitti_results)
         self._graphs = collections.OrderedDict()
         self.max_graphs = 8
         self._ovf_host = None
@@ -141,30 +140,72 @@ class InferencePipeline:
             raise ValueError("offsets[-1] = %d but points has %d rows" % (offsets[-1], n_points))
         return offsets
 
-    def _graph_entry(self, batch, n_points, ndim):
-        """The graph of (batch, bucket, ndim), least recently used last; a new entry has buffers but no graph yet."""
-        key = (batch, self.bucket_of(n_points), ndim)
+    # ---- the graph cache and the run-and-fetch loop every entry point goes through -----------------------------------
+    def _cached(self, key, make, fits=None):
+        """The graph-cache entry at `key`, marked most recently used.  A missing entry, or one `fits` rejects, is
+        replaced by make(), after evicting least recently used entries until there is room under max_graphs."""
         entry = self._graphs.get(key)
-        if entry is not None:
+        if entry is not None and (fits is None or fits(entry)):
             self._graphs.move_to_end(key)
             return entry
+        self._graphs.pop(key, None)
         while len(self._graphs) >= self.max_graphs:
             self._graphs.popitem(last=False)
-        entry = self._graphs[key] = _GraphEntry(key[1], batch, ndim, self.device)
+        entry = self._graphs[key] = make()
         return entry
+
+    def _serve(self, graphed, key, make, step, fetch, stage=None, fits=None):
+        """Runs one entry point: takes its entry (graphed: _cached(key, make, fits); eager: a transient make()), stages
+        the inputs into it (stage(entry)), runs step(entry) -- eagerly, or captured into and replayed from entry.graph
+        -- enqueues the D2H copies of fetch(entry, step's outputs), and syncs once.  When the f16-range flag was raised,
+        the model has switched to tf32x3 and check_overflow has dropped the graphs, so everything runs once more from
+        a fresh lookup.  Returns fetch's host result."""
+        for _attempt in range(2):
+            entry = self._cached(key, make, fits) if graphed else make()
+            if stage is not None:
+                stage(entry)
+            out = self._run_graph(entry, lambda: step(entry)) if graphed else step(entry)
+            host = fetch(entry, out)
+            if not self._sync_overflow():
+                break
+        return host
+
+    @staticmethod
+    def _packed_into(pinned_out):
+        """_serve's fetch of the packed detections: their D2H copy into pinned_out (allocated pinned when None)."""
+        def fetch(_entry, packed):
+            nonlocal pinned_out
+            if pinned_out is None:
+                pinned_out = torch.empty(packed.shape, dtype=torch.float32, pin_memory=True)
+            return pinned_out.copy_(packed, non_blocking=True)
+        return fetch
+
+    def _sync_overflow(self):
+        """D2H of the f16-range flag behind the copies already enqueued, then one sync.  Returns True when the flag was
+        raised and the model has switched to tf32x3 (check_overflow)."""
+        flag = self.overflow_flag()
+        if flag is not None:
+            if self._ovf_host is None:
+                self._ovf_host = torch.zeros(1, dtype=torch.int32, pin_memory=True)
+            self._ovf_host.copy_(flag, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        return flag is not None and self.check_overflow(int(self._ovf_host[0]))
+
+    def _points_entry(self, batch, bucket, ndim):
+        """forward_graphed's entry (batch, bucket, ndim): static points [bucket, ndim] and device offsets [batch + 1]."""
+        return _GraphEntry(points=torch.zeros((bucket, ndim), dtype=torch.float32, device=self.device), rows=RowStager(),
+                           offsets=_Upload(torch.zeros(batch + 1, dtype=torch.int32, device=self.device)))
+
+    def _graph_entry(self, batch, n_points, ndim):
+        """The graph-cache entry of (batch, bucket_of(n_points), ndim); a new entry has buffers but no graph yet."""
+        key = (batch, self.bucket_of(n_points), ndim)
+        return self._cached(key, lambda: self._points_entry(*key))
 
     def _replay(self, entry, offsets):
         """Make the graph's device offsets `offsets`, capture the graph on first use, replay.  The clouds must already
         be in entry.points[:offsets[-1]]."""
-        key = tuple(offsets)
-        if entry.last_offsets != key:
-            # the pinned staging buffer may still feed the previous copy: wait for that one before rewriting it
-            entry.copied.synchronize()
-            entry.staging.numpy()[:] = key
-            entry.offsets.copy_(entry.staging, non_blocking=True)
-            entry.copied.record()
-            entry.last_offsets = key
-        return self._run_graph(entry, lambda: self.pack(self.forward_device(entry.points, entry.offsets)))
+        entry.offsets.put(offsets)
+        return self._run_graph(entry, lambda: self.pack(self.forward_device(entry.points, entry.offsets.dev)))
 
     def _run_graph(self, entry, step):
         """Capture `step` (which returns the packed detections) into entry.graph on first use, then replay it."""
@@ -217,44 +258,23 @@ class InferencePipeline:
         offsets = [0]
         for c in clouds:
             offsets.append(offsets[-1] + c.shape[0])
-        ndim = clouds[0].shape[1]
+        batch, ndim = len(clouds), clouds[0].shape[1]
         if graphed:
             self.check_offsets(offsets)
-        else:
-            pts = torch.empty((offsets[-1], ndim), dtype=torch.float32, device=self.device)
-            for c, a, b in zip(clouds, offsets[:-1], offsets[1:]):
-                pts[a:b].copy_(c, non_blocking=True)
-        for _attempt in range(2):
-            if graphed:         # (a re-run after an overflow captures a new graph: check_overflow dropped them all)
-                entry = self._graph_entry(len(clouds), offsets[-1], ndim)
-                for c, a, b in zip(clouds, offsets[:-1], offsets[1:]):
-                    entry.points[a:b].copy_(c, non_blocking=True)
-                packed = self._replay(entry, offsets)
-            else:
-                packed = self.pack(self.forward_device(pts, offsets))
-            pinned_out, rerun = self._fetch(packed, pinned_out)
-            if not rerun:
-                break
-        return pinned_out
+            key = (batch, self.bucket_of(offsets[-1]), ndim)
+            make = lambda: self._points_entry(*key)                                                       # noqa: E731
+            step = lambda e: self.pack(self.forward_device(e.points, e.offsets.dev))                      # noqa: E731
+        else:           # an exactly sized buffer and host offsets
+            key = None
+            make = lambda: _GraphEntry(points=torch.empty((offsets[-1], ndim), dtype=torch.float32,      # noqa: E731
+                                                          device=self.device), rows=RowStager())
+            step = lambda e: self.pack(self.forward_device(e.points, offsets))                            # noqa: E731
 
-    def _fetch(self, packed, pinned_out):
-        """D2H of the packed detections and of the f16-range flag, then one sync.  Returns (pinned_out, rerun): rerun is
-        True when the flag was raised and the model has switched to tf32x3 (check_overflow)."""
-        if pinned_out is None:
-            pinned_out = torch.empty(packed.shape, dtype=torch.float32, pin_memory=True)
-        pinned_out.copy_(packed, non_blocking=True)
-        return pinned_out, self._sync_overflow()
-
-    def _sync_overflow(self):
-        """D2H of the f16-range flag behind the copies already enqueued, then one sync.  Returns True when the flag was
-        raised and the model has switched to tf32x3 (check_overflow)."""
-        flag = self.overflow_flag()
-        if flag is not None:
-            if self._ovf_host is None:
-                self._ovf_host = torch.zeros(1, dtype=torch.int32, pin_memory=True)
-            self._ovf_host.copy_(flag, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        return flag is not None and self.check_overflow(int(self._ovf_host[0]))
+        def stage(e):
+            e.rows.put(clouds, e.points)
+            if graphed:
+                e.offsets.put(offsets)
+        return self._serve(graphed, key, make, step, self._packed_into(pinned_out), stage)
 
     @torch.no_grad()
     def infer_sweeps(self, samples, pinned_out=None, graphed=False, n_feat=4, radius=1.0):
@@ -275,37 +295,18 @@ class InferencePipeline:
         samples = list(samples)
         stride, sizes = check_sweep_samples(samples, n_feat)
         batch, total = len(samples), sum(map(sum, sizes))
-        bucket = self.bucket_of(total)
-        table_cap = sweep_table_capacity(sum(map(len, sizes)), batch)
-        if not graphed:
-            # the voxelizer keeps its device-offset buffers per capacity: the bucket bounds how many it keeps
-            points, cloud_offsets = ingest_sweeps_batched(samples, radius, n_feat, self.device, capacity=bucket)
-        for _attempt in range(2):
-            if graphed:         # (a re-run after an overflow captures a new graph: check_overflow dropped them all)
-                entry = self._sweep_graph_entry(batch, bucket, table_cap, stride, n_feat, radius)
-                entry.stage(samples, sizes)
-                ing = entry.ingest
-                packed = self._run_graph(entry, lambda: self.pack(self.forward_device(*ing.launch())))
-            else:
-                packed = self.pack(self.forward_device(points, cloud_offsets))
-            pinned_out, rerun = self._fetch(packed, pinned_out)
-            if not rerun:
-                break
-        return pinned_out
+        key = (batch, self.bucket_of(total), sweep_table_capacity(sum(map(len, sizes)), batch), stride, n_feat)
 
-    def _sweep_graph_entry(self, batch, bucket, table_cap, raw_stride, n_feat, radius):
-        """The infer_sweeps graph of (batch, bucket, table_cap, raw_stride, n_feat), in the LRU of forward_graphed."""
-        key = (batch, bucket, table_cap, raw_stride, n_feat)
-        entry = self._graphs.get(key)
-        if entry is not None and entry.ingest.radius == radius:
-            self._graphs.move_to_end(key)
-            return entry
-        self._graphs.pop(key, None)
-        while len(self._graphs) >= self.max_graphs:
-            self._graphs.popitem(last=False)
-        entry = self._graphs[key] = _SweepGraphEntry(BatchedIngest(batch, bucket, table_cap, raw_stride, n_feat, radius,
-                                                                   self.device))
-        return entry
+        def make():
+            # eager too, the voxelizer's capacity is the bucket: it keeps its device-offset buffers per capacity
+            ingest = BatchedIngest(*key, radius, self.device)
+            return _GraphEntry(ingest=ingest, table=_Upload(ingest.table), rows=RowStager())
+
+        def stage(e):
+            e.table.put(e.ingest.host_table(samples, sizes))
+            e.rows.put([r for raws, _tms, _lags in samples for r in raws], e.ingest.raw)
+        return self._serve(graphed, key, make, lambda e: self.pack(self.forward_device(*e.ingest.launch())),
+                           self._packed_into(pinned_out), stage, fits=lambda e: e.ingest.radius == radius)
 
     # ---- raw KITTI scans: camera-frustum crop on the device ----------------------------------------------------------
     @staticmethod
@@ -398,53 +399,37 @@ class InferencePipeline:
         tables = np.stack([self.kitti_calib_table(c) for c in calibs]) if kitti_results else None
         offsets = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int32)
         batch, bucket = len(clouds), self.bucket_of(int(offsets[-1]))
-        if not graphed:
-            crop = FrustumCrop(batch, bucket, ndim, self.device)
-            _stage_clouds(clouds, offsets, crop.points)
-            crop.set_table(offsets, planes)
-            points, cloud_offsets = crop.launch()
-            if kitti_results:
-                kitti = KittiResults(batch, self.device)
-                kitti.set_calib(tables)
-        for _attempt in range(2):
-            if graphed:         # (a re-run after an overflow captures a new graph: check_overflow dropped them all)
-                entry = self._frustum_graph_entry(batch, bucket, ndim, kitti_results)
-                entry.stage(clouds, offsets, planes, tables)
-                crop, kitti = entry.crop, entry.kitti
-                if kitti_results:
-                    step = lambda: kitti.launch(self.pack(self.forward_device(*crop.launch())))   # noqa: E731
-                else:
-                    step = lambda: self.pack(self.forward_device(*crop.launch()))                 # noqa: E731
-                out = self._run_graph(entry, step)
-            else:
-                out = self.pack(self.forward_device(points, cloud_offsets))
-                if kitti_results:
-                    out = kitti.launch(out)
-            if kitti_results:
-                kitti.results_host.copy_(out[0], non_blocking=True)
-                kitti.counts_host.copy_(out[1], non_blocking=True)
-                rerun = self._sync_overflow()
-            else:
-                pinned_out, rerun = self._fetch(out, pinned_out)
-            if not rerun:
-                break
-        if kitti_results:
-            return to_annos(kitti.results_host.numpy(), kitti.counts_host.numpy(), self.class_names())
-        return pinned_out
 
-    def _frustum_graph_entry(self, batch, bucket, ndim, kitti_results=False):
-        """The infer_raw graph of ("frustum", batch, bucket, ndim) (kitti_results: ("frustum_kitti", ...), whose entry
-        also holds a KittiResults), in the LRU of forward_graphed."""
+        def make():
+            crop = FrustumCrop(batch, bucket, ndim, self.device)
+            kitti = KittiResults(batch, self.device) if kitti_results else None
+            return _GraphEntry(crop=crop, offsets=_Upload(crop.offsets), planes=_Upload(crop.planes), rows=RowStager(),
+                               kitti=kitti, calib=None if kitti is None else _Upload(kitti.calib),
+                               planes_uploads=0, calib_uploads=0)          # H2D copies of each table so far
+
+        def stage(e):
+            e.rows.put(clouds, e.crop.points)
+            e.offsets.put(offsets)
+            e.planes_uploads += e.planes.put(planes)
+            if e.kitti is not None:
+                e.calib_uploads += e.calib.put(tables)
+
+        def step(e):
+            packed = self.pack(self.forward_device(*e.crop.launch()))
+            return packed if e.kitti is None else e.kitti.launch(packed)
+
+        def fetch(e, out):
+            if e.kitti is None:
+                return packed_into(e, out)
+            e.kitti.results_host.copy_(out[0], non_blocking=True)
+            e.kitti.counts_host.copy_(out[1], non_blocking=True)
+            return e.kitti
+        packed_into = self._packed_into(pinned_out)
         key = ("frustum_kitti" if kitti_results else "frustum", batch, bucket, ndim)
-        entry = self._graphs.get(key)
-        if entry is not None:
-            self._graphs.move_to_end(key)
-            return entry
-        while len(self._graphs) >= self.max_graphs:
-            self._graphs.popitem(last=False)
-        kitti = KittiResults(batch, self.device) if kitti_results else None
-        entry = self._graphs[key] = _FrustumGraphEntry(FrustumCrop(batch, bucket, ndim, self.device), kitti)
-        return entry
+        got = self._serve(graphed, key, make, step, fetch, stage)
+        if kitti_results:
+            return to_annos(got.results_host.numpy(), got.counts_host.numpy(), self.class_names())
+        return got
 
     @staticmethod
     def unpack(packed_host):
@@ -457,115 +442,39 @@ class InferencePipeline:
 
 
 class _GraphEntry:
-    """Static buffers of one captured forward: points [bucket, ndim], device offsets [batch + 1] and their pinned
-    staging copy, the graph and its packed output."""
+    """One entry point's state: the static buffers it attaches (points, a BatchedIngest, a FrustumCrop, a KittiResults,
+    their _Uploads and RowStager) and, once captured, the graph and its output.  A graphed entry lives in the graph
+    cache; an eager one serves one call."""
 
-    def __init__(self, bucket, batch, ndim, device):
-        self.points = torch.zeros((bucket, ndim), dtype=torch.float32, device=device)
-        self.offsets = torch.zeros(batch + 1, dtype=torch.int32, device=device)
-        self.staging = torch.zeros(batch + 1, dtype=torch.int32, pin_memory=True)
+    def __init__(self, **buffers):
+        self.graph = self.out = None
+        self.__dict__.update(buffers)
+
+
+class _Upload:
+    """A small device table `dev` that goes H2D only when its bytes change, through a pinned staging copy."""
+
+    def __init__(self, dev):
+        self.dev = dev
+        self.staging = torch.empty(dev.shape, dtype=dev.dtype, pin_memory=True)
         self.copied = torch.cuda.Event()
-        self.last_offsets = None
-        self.graph = None
-        self.out = None
+        self.last = None
 
-
-class _SweepGraphEntry:
-    """Static buffers of one captured infer_sweeps forward: the BatchedIngest (raw sweeps, sweep table, clouds, cloud
-    offsets), the pinned staging of the table and of raw sweeps that are not pinned already, the graph and its output."""
-
-    def __init__(self, ingest):
-        self.ingest = ingest
-        self.table_staging = torch.zeros(ingest.table.numel(), dtype=torch.uint8, pin_memory=True)
-        self.raw_staging = None
-        self.copied = torch.cuda.Event()
-        self.last_table = None
-        self.graph = None
-        self.out = None
-
-    def stage(self, samples, sizes):
-        """Enqueue the H2D copies of the raw sweeps and, when it differs from the previous replay's, of the table."""
-        # the pinned staging buffers may still feed the previous copies: wait for those before rewriting them
-        self.copied.synchronize()
-        table = self.ingest.host_table(samples, sizes)
-        if self.last_table is None or not np.array_equal(table, self.last_table):
-            self.table_staging.numpy()[:] = table
-            self.ingest.table.copy_(self.table_staging, non_blocking=True)
-            self.last_table = table
-        if self.raw_staging is None and not all(torch.is_tensor(r) and r.is_pinned() for s in samples for r in s[0]):
-            self.raw_staging = torch.empty(self.ingest.raw.shape, dtype=torch.float32, pin_memory=True)
-        stage_raw_sweeps(samples, sizes, self.ingest.raw, self.raw_staging)
-        self.copied.record()
-
-
-def _stage_clouds(clouds, offsets, points_dev, staging=None):
-    """Enqueues the H2D copies of the clouds into points_dev[offsets[b]:offsets[b + 1]].  Pinned tensors are copied
-    directly; anything else goes through the pinned `staging` buffer (allocated like points_dev when None).  Returns
-    the staging buffer."""
-    for c, a, b in zip(clouds, offsets[:-1], offsets[1:]):
-        if b > a:
-            src = c if torch.is_tensor(c) and c.is_pinned() else None
-            if src is None:
-                if staging is None:
-                    staging = torch.empty(points_dev.shape, dtype=torch.float32, pin_memory=True)
-                src = staging[a:b]
-                src.copy_(torch.as_tensor(c))
-            points_dev[a:b].copy_(src, non_blocking=True)
-    return staging
-
-
-class _FrustumGraphEntry:
-    """Static buffers of one captured infer_raw forward: the FrustumCrop (raw scans, offsets, planes, cropped clouds,
-    their offsets), with kitti_results the KittiResults (calibration table, result rows, counts), the pinned staging of
-    the offsets, of the planes, of the calibration table and of scans that are not pinned already, the graph and its
-    output."""
-
-    def __init__(self, crop, kitti=None):
-        self.crop, self.kitti = crop, kitti
-        self.offsets_staging = torch.zeros(crop.offsets.shape, dtype=torch.int32, pin_memory=True)
-        self.planes_staging = torch.zeros(crop.planes.shape, dtype=torch.float64, pin_memory=True)
-        self.calib_staging = None if kitti is None else torch.zeros(kitti.calib.shape, dtype=torch.float64,
-                                                                     pin_memory=True)
-        self.raw_staging = None
-        self.copied = torch.cuda.Event()
-        self.last_offsets = self.last_planes = self.last_calib = None
-        self.planes_uploads = 0                   # plane-table H2D copies so far
-        self.calib_uploads = 0                    # KITTI calibration-table H2D copies so far
-        self.graph = None
-        self.out = None
-
-    def stage(self, clouds, offsets, planes, calib_table=None):
-        """Enqueue the H2D copies of the scans and, when they differ from the previous replay's, of the offsets, of
-        the plane table and of the KITTI calibration table."""
-        # the pinned staging buffers may still feed the previous copies: wait for those before rewriting them
-        self.copied.synchronize()
-        crop = self.crop
-        if self.last_offsets is None or not np.array_equal(offsets, self.last_offsets):
-            self.offsets_staging.numpy()[:] = offsets
-            crop.offsets.copy_(self.offsets_staging, non_blocking=True)
-            self.last_offsets = offsets.copy()
-        if self.last_planes is None or not np.array_equal(planes.view(np.uint64), self.last_planes.view(np.uint64)):
-            self.planes_staging.numpy()[:] = planes
-            crop.planes.copy_(self.planes_staging, non_blocking=True)
-            self.last_planes = planes.copy()
-            self.planes_uploads += 1
-        if self.kitti is not None and (self.last_calib is None or not np.array_equal(
-                calib_table.view(np.uint64), self.last_calib.view(np.uint64))):
-            self.calib_staging.numpy()[:] = calib_table
-            self.kitti.calib.copy_(self.calib_staging, non_blocking=True)
-            self.last_calib = calib_table.copy()
-            self.calib_uploads += 1
-        self.raw_staging = _stage_clouds(clouds, offsets, crop.points, self.raw_staging)
-        self.copied.record()
-
-
-class _StreamGraphEntry:
-    """One captured SweepStream forward: the stream whose buffers the graph holds, the graph and its packed output."""
-
-    def __init__(self, stream):
-        self.stream = stream
-        self.graph = None
-        self.out = None
+    def put(self, value, always=False):
+        """Enqueues the H2D copy of the host `value` (dev's shape, converted to its dtype) unless its bytes equal the
+        last put's; always=True copies in any case.  Returns whether it copied."""
+        host = self.staging.numpy()
+        value = np.asarray(value, host.dtype)
+        raw = value.tobytes()
+        if raw == self.last and not always:
+            return False
+        self.copied.synchronize()                 # the staging buffer may still feed the previous copy
+        host[...] = value
+        with torch.cuda.device(self.dev.device):
+            self.dev.copy_(self.staging, non_blocking=True)
+            self.copied.record()
+        self.last = raw
+        return True
 
 
 class SweepStream:
@@ -610,8 +519,6 @@ class SweepStream:
         self.pending_h2d_bytes = 0                # pushed since the last infer()
         self.last_h2d_bytes = 0                   # of the last infer(): the pushes before it + its table
         self._ingest = None                       # device buffers, allocated on the first push
-        self._push_staging = None                 # pinned [B, slot_capacity, raw_stride], allocated on first need
-        self._push_copied = None
 
     def _buffers(self):
         """The gather BatchedIngest whose raw buffer holds the slots, and the slots' [B, K, slot_capacity, raw_stride]
@@ -621,8 +528,8 @@ class SweepStream:
             self._ingest = BatchedIngest(B, B * K * self.slot_capacity, B * K, self.raw_stride, self.n_feat, self.radius,
                                          self.pipe.device, gather=True)
             self._slots = self._ingest.raw.view(B, K, self.slot_capacity, self.raw_stride)
-            self._table_staging = torch.zeros(self._ingest.table.numel(), dtype=torch.uint8, pin_memory=True)
-            self._table_copied = torch.cuda.Event()
+            self._table = _Upload(self._ingest.table)
+            self._rows = [RowStager() for _ in range(B)]            # one staging buffer [slot_capacity] per stream
         return self._ingest, self._slots
 
     def check_push(self, b, raw, pose, timestamp):
@@ -651,22 +558,7 @@ class SweepStream:
         is enqueued when an argument is malformed."""
         rows = self.check_push(b, raw, pose, timestamp)
         _ing, slots = self._buffers()
-        slot = self.sweeps.next_slot(b)
-        if rows:
-            with torch.cuda.device(slots.device):
-                src = raw if torch.is_tensor(raw) and raw.is_pinned() else None
-                if src is None:
-                    if self._push_staging is None:
-                        self._push_staging = torch.empty((self.batch, self.slot_capacity, self.raw_stride),
-                                                         dtype=torch.float32, pin_memory=True)
-                        self._push_copied = [torch.cuda.Event() for _ in range(self.batch)]
-                    self._push_copied[b].synchronize()          # stream b's staging may still feed its previous copy
-                    src = self._push_staging[b, :rows]
-                    src.copy_(torch.as_tensor(raw))
-                    slots[b, slot, :rows].copy_(src, non_blocking=True)
-                    self._push_copied[b].record()
-                else:
-                    slots[b, slot, :rows].copy_(src, non_blocking=True)
+        self._rows[b].put([raw], slots[b, self.sweeps.next_slot(b)])
         self.sweeps.record(b, rows, pose, timestamp)
         self.pending_h2d_bytes += rows * self.raw_stride * 4
 
@@ -683,31 +575,15 @@ class SweepStream:
                 for b, (ks, ns, tms, lags) in enumerate(frame)]
 
     def _stage_table(self):
-        """Writes the current frame's sweep table into the pinned staging buffer and enqueues its H2D copy."""
+        """Enqueues the H2D copy of the current frame's sweep table (every frame: it changes with each push)."""
         frame = self.sweeps.frame()
         ing, _slots = self._buffers()
         K, cap = self.history, self.slot_capacity
         src = [(b * K + k) * cap for b, (ks, _ns, _tms, _lags) in enumerate(frame) for k in ks]
-        self._table_copied.synchronize()          # the staging buffer may still feed the previous frame's copy
-        ing.host_table([(None, tms, lags) for _ks, _ns, tms, lags in frame], [ns for _ks, ns, _tms, _lags in frame],
-                       out=self._table_staging.numpy(), sweep_src=src)
-        with torch.cuda.device(ing.table.device):
-            ing.table.copy_(self._table_staging, non_blocking=True)
-            self._table_copied.record()
+        self._table.put(ing.host_table([(None, tms, lags) for _ks, _ns, tms, lags in frame],
+                                       [ns for _ks, ns, _tms, _lags in frame], sweep_src=src), always=True)
         self.last_h2d_bytes = self.pending_h2d_bytes + ing.table.numel()
         self.pending_h2d_bytes = 0
-
-    def _graph_entry(self):
-        graphs = self.pipe._graphs
-        entry = graphs.get(self.key)
-        if entry is not None and entry.stream is self:
-            graphs.move_to_end(self.key)
-            return entry
-        graphs.pop(self.key, None)
-        while len(graphs) >= self.pipe.max_graphs:
-            graphs.popitem(last=False)
-        entry = graphs[self.key] = _StreamGraphEntry(self)
-        return entry
 
     @torch.no_grad()
     def infer(self, pinned_out=None, graphed=False):
@@ -716,14 +592,7 @@ class SweepStream:
         stream's CUDA graph.  On an f16-range overflow the model switches to tf32x3 and the same frame is re-run, as in
         infer_sweeps; the history is not touched.  ValueError when a stream holds no sweep."""
         self._stage_table()
-        pipe, ing = self.pipe, self._ingest
-        step = lambda: pipe.pack(pipe.forward_device(*ing.launch()))      # noqa: E731
-        for _attempt in range(2):
-            if graphed:         # (a re-run after an overflow captures a new graph: check_overflow dropped them all)
-                packed = pipe._run_graph(self._graph_entry(), step)
-            else:
-                packed = step()
-            pinned_out, rerun = pipe._fetch(packed, pinned_out)
-            if not rerun:
-                break
-        return pinned_out
+        pipe = self.pipe
+        return pipe._serve(graphed, self.key, lambda: _GraphEntry(stream=self),
+                           lambda e: pipe.pack(pipe.forward_device(*self._ingest.launch())),
+                           pipe._packed_into(pinned_out), fits=lambda e: e.stream is self)

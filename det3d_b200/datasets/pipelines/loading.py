@@ -237,22 +237,46 @@ class SweepHistory:
         return out
 
 
-def stage_raw_sweeps(samples, sizes, raw_dev, staging=None):
-    """Enqueues the H2D copies of every raw sweep into raw_dev, back to back in sample order.  Pinned tensors are copied
-    directly; anything else goes through the pinned `staging` buffer ([>= total, raw_stride], allocated when None)."""
-    at = 0
-    for (raws, _tms, _lags), n in zip(samples, sizes):
-        for r, k in zip(raws, n):
-            if k:
-                src = r if torch.is_tensor(r) and r.is_pinned() else None
-                if src is None:
-                    if staging is None:
-                        staging = torch.empty(raw_dev.shape, dtype=torch.float32, pin_memory=True)
-                    src = staging[at:at + k]
-                    src.copy_(torch.as_tensor(r))
-                raw_dev[at:at + k].copy_(src, non_blocking=True)
-            at += k
-    return at
+class RowStager:
+    """H2D copies of host row arrays into device rows.  Pinned tensors are copied directly; anything else goes through
+    a pinned staging buffer shaped like the device rows, allocated on first need.  The staging buffer may still feed
+    the previous put's copies when the next put rewrites it, so each put waits for those first (its own event)."""
+
+    def __init__(self):
+        self.staging = None
+        self.copied = None
+
+    def put(self, arrays, dst):
+        """Enqueues the H2D copies of `arrays` (float32 [n_i, dst.shape[1]] host arrays or tensors) back to back into
+        the device rows dst[0:sum(n_i)]; every put of one stager has dst of the same shape.  Returns sum(n_i)."""
+        at, staged = 0, False
+        with torch.cuda.device(dst.device):
+            for a in arrays:
+                k = int(a.shape[0])
+                if not k:
+                    continue
+                src = a
+                if not (torch.is_tensor(a) and a.is_pinned()):
+                    if self.staging is None:
+                        self.staging = torch.empty(dst.shape, dtype=torch.float32, pin_memory=True)
+                        self.copied = torch.cuda.Event()
+                    if not staged:
+                        self.copied.synchronize()
+                        staged = True
+                    src = self.staging[at:at + k]
+                    src.copy_(torch.as_tensor(a))
+                dst[at:at + k].copy_(src, non_blocking=True)
+                at += k
+            if staged:
+                self.copied.record()
+        return at
+
+
+def stage_raw_sweeps(samples, sizes, raw_dev):
+    """Enqueues the H2D copies of every raw sweep into raw_dev, back to back in sample order, through a RowStager of
+    its own.  `sizes` (check_sweep_samples') is not read: each array's shape gives its rows.  Returns the number of
+    rows."""
+    return RowStager().put([r for raws, _tms, _lags in samples for r in raws], raw_dev)
 
 
 class BatchedIngest:
