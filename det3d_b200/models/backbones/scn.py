@@ -111,39 +111,35 @@ class _SparseMiddleEncoder(nn.Module):
             self._fused = spconv.FusedSparseEncoder(self.middle_conv)
         return self._fused
 
-    def forward(self, voxel_features, coors, batch_size, input_shape, n_dev=None):
-        """-> dense BEV features [B, C*D, H, W] (scn.py:184-197).
-
-        `n_dev` (optional int32 device tensor) marks how many leading rows of
-        voxel_features / coors are live, for the sync-free fused pipeline."""
-        if self.training:
-            raise RuntimeError("det3d_b200 middle encoders are inference-only: call .eval()")
-        sparse_shape = [int(v) for v in (np.array(input_shape[::-1]) + [1, 0, 0])]
-        dense = self.fused().run(voxel_features, coors.int(), int(batch_size), sparse_shape, n_dev=n_dev)
-        n, c, d, h, w = dense.shape
-        return dense.view(n, c * d, h, w)
-
-    def forward_rows(self, voxel_features, coors, batch_size, input_shape, n_dev=None):
-        """Channels-last variant: (rows [B*H*W, C*D], (B, H, W)); rows.view(B,H,W,-1).permute(0,3,1,2)
-        equals forward()'s [B, C*D, H, W]."""
-        if self.training:
-            raise RuntimeError("det3d_b200 middle encoders are inference-only: call .eval()")
-        sparse_shape = [int(v) for v in (np.array(input_shape[::-1]) + [1, 0, 0])]
-        fused = self.fused()
-        rows = fused.run(voxel_features, coors.int(), int(batch_size), sparse_shape, n_dev=n_dev, bev_rows=True)
-        _d, h, w = fused._state["final_level"].spatial
-        return rows, (int(batch_size), h, w)
-
-    def forward_planes(self, voxel_features, coors, batch_size, input_shape, n_dev=None, overflow=None):
-        """NHWC split-f16 planes [B, H, W, C*D] of the BEV map (the FP16x3 dense path's input): the same values as
-        forward()'s [B, C*D, H, W]."""
+    def _encode(self, voxel_features, coors, batch_size, input_shape, n_dev, overflow, bev_rows):
         if self.training:
             raise RuntimeError("det3d_b200 middle encoders are inference-only: call .eval()")
         sparse_shape = [int(v) for v in (np.array(input_shape[::-1]) + [1, 0, 0])]
         fused = self.fused()
         if overflow is not None:
             fused.external_overflow = overflow
-        return fused.run(voxel_features, coors.int(), int(batch_size), sparse_shape, n_dev=n_dev, bev_rows="planes")
+        return fused.run(voxel_features, coors.int(), int(batch_size), sparse_shape, n_dev=n_dev, bev_rows=bev_rows)
+
+    def forward(self, voxel_features, coors, batch_size, input_shape, n_dev=None):
+        """-> dense BEV features [B, C*D, H, W] (scn.py:184-197).
+
+        `n_dev` (optional int32 device tensor) marks how many leading rows of
+        voxel_features / coors are live, for the sync-free fused pipeline."""
+        dense = self._encode(voxel_features, coors, batch_size, input_shape, n_dev, None, False)
+        n, c, d, h, w = dense.shape
+        return dense.view(n, c * d, h, w)
+
+    def forward_rows(self, voxel_features, coors, batch_size, input_shape, n_dev=None, overflow=None):
+        """Channels-last fp32 BEV features [B, H, W, C*D] (the tf32x3 dense path's input): the same values as
+        forward()'s [B, C*D, H, W]."""
+        rows = self._encode(voxel_features, coors, batch_size, input_shape, n_dev, overflow, True)
+        _d, h, w = self.fused()._state["final_level"].spatial
+        return rows.view(int(batch_size), h, w, rows.shape[1])
+
+    def forward_planes(self, voxel_features, coors, batch_size, input_shape, n_dev=None, overflow=None):
+        """NHWC split-f16 planes [B, H, W, C*D] of the BEV map (the FP16x3 dense path's input): the same values as
+        forward()'s [B, C*D, H, W]."""
+        return self._encode(voxel_features, coors, batch_size, input_shape, n_dev, overflow, "planes")
 
     def forward_unfused(self, voxel_features, coors, batch_size, input_shape):
         """Layer-by-layer path through the spconv-style modules (API parity / cross-check)."""

@@ -45,8 +45,6 @@ class _FusedBevMixin:
     use_fused_bev = True
     math = "fp16x3"
     fp16_enabled = False        # set by det3d.core.fp16.wrap_fp16_model
-    _bev16 = None
-    _bev32 = None
     _ovf = None
 
     def set_math(self, math):
@@ -76,15 +74,17 @@ class _FusedBevMixin:
         if self.training or not self.with_neck or not self.use_fused_bev:
             return None
         from det3d_b200.ops.spconv import bev
-        if self.math in F16_MATHS:
-            if self._bev16 is None:
+        cache = self.__dict__.setdefault("_fused_bev", {})     # math family -> executor, or None: the torch modules run
+        family = "f16" if self.math in F16_MATHS else "tf32x3"
+        if family not in cache:
+            if family == "f16":
                 ok = hasattr(self.backbone, "forward_planes") and bev.rpn_is_fusable16(self.neck)
-                self._bev16 = bev.FusedBevStack(self.neck, self.bbox_head) if ok else False
-            return self._bev16 or None
-        if self._bev32 is None:
-            ok = hasattr(self.backbone, "forward_rows") and bev.rpn_is_fusable(self.neck)
-            self._bev32 = bev.FusedBevStackTF32(self.neck, self.bbox_head) if ok else False
-        return self._bev32 or None
+                stack = bev.FusedBevStack
+            else:
+                ok = hasattr(self.backbone, "forward_rows") and bev.rpn_is_fusable(self.neck)
+                stack = bev.FusedBevStackTF32
+            cache[family] = stack(self.neck, self.bbox_head) if ok else None
+        return cache[family]
 
 
 @DETECTORS.register_module
@@ -102,17 +102,15 @@ class VoxelNet(_FusedBevMixin, SingleStageDetector):
                     coors=example["coordinates"], batch_size=len(num_voxels),
                     input_shape=example["shape"][0], n_dev=example.get("n_voxels_dev"))
         bev = self.fused_bev() if not return_loss else None
-        if bev is not None and self.math in F16_MATHS:
+        if bev is not None:
             feats = self.reader(data["features"], data["num_voxels"])
-            ovf = self.overflow_flag(feats.device)
-            planes = self.backbone.forward_planes(feats, data["coors"], data["batch_size"], data["input_shape"],
-                                                  n_dev=data["n_dev"], overflow=ovf)
-            preds = bev.run(planes, overflow=ovf)
-        elif bev is not None:
-            feats = self.reader(data["features"], data["num_voxels"])
-            rows, (b, h, w) = self.backbone.forward_rows(feats, data["coors"], data["batch_size"],
-                                                          data["input_shape"], n_dev=data["n_dev"])
-            preds = bev.run(rows, b, h, w)
+            # the BEV map in the form the math's stack takes: f16 planes, or fp32 channels-last features
+            f16 = self.math in F16_MATHS
+            ovf = self.overflow_flag(feats.device) if f16 else None
+            bev_input = self.backbone.forward_planes if f16 else self.backbone.forward_rows
+            x = bev_input(feats, data["coors"], data["batch_size"], data["input_shape"], n_dev=data["n_dev"],
+                          overflow=ovf)
+            preds = bev.run(x, overflow=ovf)
         else:
             preds = self.bbox_head(self.extract_feat(data))
         if return_loss:

@@ -1,17 +1,13 @@
-"""Channels-last dense BEV convolutions through the sparse-conv tensor-core kernel.
+"""Fused RPN + heads executors on the BEV map: the reference's RPN (det3d/models/necks/rpn.py:82-159) and the
+MultiGroupHead convs (det3d/models/bbox_heads/mg_head.py:198-230) with BN / ReLU folded into each conv's epilogue.
 
-The reference's RPN (det3d/models/necks/rpn.py:124-159: ZeroPad+conv3x3, N x conv3x3, each
-followed by BN2d + ReLU, then a 1x1 "deblock") and the MultiGroupHead 1x1 convs
-(det3d/models/bbox_heads/mg_head.py:198-230) are dense stride-1 convolutions over the
-[B, 200, 176] BEV grid.  In channels-last layout a dense conv IS the gather-GEMM the sparse
-kernel already performs, with a static rulebook (d3b_rulebook_dense2d: neighbour = row +- 1,
-+- W, -1 at the border = zero padding).  So the same tensor-core 3xTF32 kernel -- fp32-equivalent
-accuracy, BN/ReLU folded into its epilogue -- replaces fp32 cuDNN here, and the head's three
-1x1 convs become ONE conv whose [B*H*W, 32] output rows are already the NHWC-permuted layout
+`FusedBevStack` (fp16x3 / fp16) takes every RPN the reference builds, on NHWC f16 planes through TMA tensor maps
+(csrc/bevconv16_sm90.cu).  `FusedBevStackTF32` (tf32x3: the re-run after an f16-range overflow) takes the stride-1 /
+1x1-deblock RPN shape (the SECOND configs) through the 3xTF32 sparse-conv kernel: in channels-last layout a dense
+stride-1 conv IS the gather-GEMM that kernel performs, with a static rulebook (d3b_rulebook_dense2d: neighbour = row
++- 1, +- W, -1 at the border = zero padding); any other RPN stays on the module's regular torch forward under tf32x3.
+In both, the heads of all tasks are ONE 1x1 conv whose fp32 output rows are already the NHWC-permuted layout
 `Head.forward` produces with `.permute(0, 2, 3, 1)`.
-
-Only the stride-1 / 1x1-deblock RPN shape (the SECOND configs) is taken; anything else
-(strided blocks, ConvTranspose deblocks) stays on the module's regular torch forward.
 """
 import ctypes as C
 
@@ -19,7 +15,7 @@ import torch
 from torch import nn
 
 from ... import _lib
-from . import core
+from . import conv16, core
 from .fused import _bn_fold
 
 
@@ -79,118 +75,6 @@ def rpn_is_fusable(rpn):
         return False
 
 
-class FusedBevStackTF32:
-    """Round-1 path (3xTF32 through the sparse gather kernel, stride-1 RPN only); kept as the fallback when a
-    feature leaves the f16 range and as an in-library cross-check of `FusedBevStack`."""
-
-    def __init__(self, rpn, head):
-        self.rpn, self.head = rpn, head
-        self._grid = None
-        self._layers = None
-        self._sig = None
-        self._bufs = {}
-
-    def _signature(self):
-        ts = [p for p in self.rpn.parameters()] + [b for b in self.rpn.buffers()] + [p for p in self.head.tasks.parameters()]
-        return tuple((t._version, t.data_ptr()) for t in ts)
-
-    def _compile(self, device):
-        layers = []  # (ConvWeights, (kh, kw, ph, pw))
-        seq = list(self.rpn.blocks[0]) + list(self.rpn.deblocks[0])
-        i = 0
-        pending_pad = 0
-        while i < len(seq):
-            m = seq[i]
-            if isinstance(m, nn.ZeroPad2d):
-                pending_pad = int(m.padding[0])
-                i += 1
-                continue
-            if isinstance(m, nn.Conv2d):
-                bn = seq[i + 1] if i + 1 < len(seq) and isinstance(seq[i + 1], nn.modules.batchnorm._BatchNorm) else None
-                relu = any(isinstance(x, nn.ReLU) for x in seq[i + 1:i + 3])
-                if bn is not None and bn.training:
-                    raise RuntimeError("fused BEV stack is inference-only: call .eval()")
-                scale = shift = None
-                if bn is not None:
-                    scale, shift = _bn_fold(bn)
-                    scale, shift = scale.to(device), shift.to(device)
-                kh, kw = m.kernel_size
-                ph, pw = int(m.padding[0]) + pending_pad, int(m.padding[1]) + pending_pad
-                pending_pad = 0
-                cw = core.ConvWeights(_conv2d_weight(m).to(device), bias=None if m.bias is None else m.bias.to(device),
-                                      scale=scale, shift=shift, relu=relu, algo=_lib.ALGO_TC)
-                layers.append((cw, (kh, kw, ph, pw)))
-                i += 1 + (1 if bn is not None else 0) + (1 if relu else 0)
-                continue
-            i += 1
-        # heads: one conv over the concatenated output channels, padded to a supported width
-        ws, bs, self._splits = [], [], []
-        for task in self.head.tasks:
-            parts = [("box_preds", task.conv_box), ("cls_preds", task.conv_cls)]
-            if task.use_dir:
-                parts.append(("dir_cls_preds", task.conv_dir))
-            names = []
-            for name, conv in parts:
-                ws.append(_conv2d_weight(conv))
-                bs.append(conv.bias.detach().float())
-                names.append((name, conv.out_channels))
-            self._splits.append(names)
-        w = torch.cat(ws, dim=2)
-        b = torch.cat(bs)
-        total = w.shape[2]
-        width = next(c for c in (16, 32, 64, 128) if c >= total)
-        w = torch.cat([w, w.new_zeros((1, w.shape[1], width - total))], dim=2)
-        b = torch.cat([b, b.new_zeros(width - total)])
-        layers.append((core.ConvWeights(w.to(device), bias=b.to(device), relu=False, algo=_lib.ALGO_TC), (1, 1, 0, 0)))
-        self._layers = layers
-
-    def _buf(self, n, c, busy, device):
-        pool = self._bufs.setdefault((n, c), [])
-        for t in pool:
-            if t is not busy:
-                return t
-        t = torch.empty((n, c), dtype=torch.float32, device=device)
-        pool.append(t)
-        return t
-
-    def run(self, rows, batch, height, width):
-        with _lib.on_device_of(rows):
-            return self._run(rows, batch, height, width)
-
-    def _run(self, rows, batch, height, width):
-        """rows [B*H*W, C] channels-last BEV features -> list (per task) of dicts like Head.forward:
-        box_preds [B,H,W,a*code], cls_preds [B,H,W,a*cls], dir_cls_preds [B,H,W,a*2]."""
-        device = rows.device
-        if self._grid is None or (self._grid.batch, self._grid.h, self._grid.w) != (batch, height, width):
-            self._grid = BevGrid(batch, height, width, device)
-        sig = self._signature()
-        if self._layers is None or sig != self._sig:
-            self._compile(device)
-            self._sig = sig
-        x = rows
-        for cw, geom in self._layers:
-            rb = self._grid.rulebook(*geom)
-            out = self._buf(self._grid.n_rows, cw.c_out, x, device)
-            core.sparse_conv(x, rb, cw, out)
-            x = out
-        preds, col = [], 0
-        flat = x.view(batch, height, width, x.shape[1])
-        for names in self._splits:
-            d = {}
-            for name, c in names:
-                d[name] = flat[..., col:col + c]
-                col += c
-            preds.append(d)
-        return preds
-
-
-# ======================================================================================================
-# FP16x3 path: the whole RPN (any block strides / ConvTranspose deblocks / concat) + all task heads on
-# NHWC f16 planes through TMA tensor maps (csrc/bevconv16_sm90.cu).
-# ======================================================================================================
-from . import conv16  # noqa: E402
-
-
 def _conv_bn_relu(seq, i):
     """(conv, bn | None, relu, next index) for the conv module at seq[i]."""
     conv = seq[i]
@@ -205,12 +89,133 @@ def _conv_bn_relu(seq, i):
     return conv, bn, relu, j
 
 
-def _layer16(conv, bn, relu, extra_pad, device):
-    if bn is not None and bn.training:
+def _convs(seq):
+    """(conv, bn | None, relu, extra padding) of each Conv2d in `seq`; a ZeroPad2d pads the conv after it."""
+    out, i, pad = [], 0, 0
+    while i < len(seq):
+        if isinstance(seq[i], nn.ZeroPad2d):
+            pad = int(seq[i].padding[0])
+            i += 1
+        elif isinstance(seq[i], nn.Conv2d):
+            conv, bn, relu, i = _conv_bn_relu(seq, i)
+            out.append((conv, bn, relu, pad))
+            pad = 0
+        else:
+            i += 1
+    return out
+
+
+def _folded_bn(bn):
+    """(scale, shift) of a BatchNorm in eval mode, or (None, None) without one."""
+    if bn is None:
+        return None, None
+    if bn.training:
         raise RuntimeError("fused BEV stack is inference-only: call .eval()")
-    scale = shift = None
-    if bn is not None:
-        scale, shift = _bn_fold(bn)
+    return _bn_fold(bn)
+
+
+class _BevStack:
+    """What both stacks share: the parameter signature their device weights were made from, the heads of every task as
+    one 1x1 conv, and the split of its output columns into one dict per task."""
+
+    def __init__(self, rpn, head):
+        self.rpn, self.head = rpn, head
+        self._sig = None
+        self._plan = None
+        self._bufs = {}
+
+    def _signature(self):
+        ts = [p for p in self.rpn.parameters()] + [b for b in self.rpn.buffers()] + [p for p in self.head.tasks.parameters()]
+        return tuple((t._version, t.data_ptr()) for t in ts)
+
+    def _compiled(self, device):
+        """The stack's device weights (its _compile), made again whenever a parameter has changed."""
+        sig = self._signature()
+        if self._plan is None or sig != self._sig:
+            self._plan = self._compile(device)
+            self._sig = sig
+        return self._plan
+
+    def _heads(self):
+        """(weight [1, C_in, C_total], bias [C_total]) of every task's box / cls / dir convs as one 1x1 conv."""
+        ws, bs, self._splits = [], [], []
+        for task in self.head.tasks:
+            parts = [("box_preds", task.conv_box), ("cls_preds", task.conv_cls)]
+            if task.use_dir:
+                parts.append(("dir_cls_preds", task.conv_dir))
+            names = []
+            for name, conv in parts:
+                ws.append(_conv2d_weight(conv))
+                bs.append(conv.bias.detach().float())
+                names.append((name, conv.out_channels))
+            self._splits.append(names)
+        return torch.cat(ws, dim=2), torch.cat(bs)
+
+    def _split(self, out):
+        """Head output [B, H, W, >= C_total] -> list (per task) of dicts like Head.forward: box_preds [B,H,W,a*code],
+        cls_preds [B,H,W,a*cls], dir_cls_preds [B,H,W,a*2] (views of `out`)."""
+        preds, c0 = [], 0
+        for names in self._splits:
+            d = {}
+            for name, c in names:
+                d[name] = out[..., c0:c0 + c]
+                c0 += c
+            preds.append(d)
+        return preds
+
+
+class FusedBevStackTF32(_BevStack):
+    """tf32x3: the stride-1 RPN and the heads through the 3xTF32 gather kernel over dense rulebooks; also an in-library
+    cross-check of `FusedBevStack`."""
+    _grid = None
+
+    def _compile(self, device):
+        to = lambda t: None if t is None else t.to(device)
+        layers = []  # (ConvWeights, (kh, kw, ph, pw))
+        for conv, bn, relu, pad in _convs(list(self.rpn.blocks[0]) + list(self.rpn.deblocks[0])):
+            scale, shift = _folded_bn(bn)
+            cw = core.ConvWeights(_conv2d_weight(conv).to(device), bias=to(conv.bias), scale=to(scale), shift=to(shift),
+                                  relu=relu, algo=_lib.ALGO_TC)
+            kh, kw = conv.kernel_size
+            layers.append((cw, (kh, kw, int(conv.padding[0]) + pad, int(conv.padding[1]) + pad)))
+        # the heads, padded with zero columns to a width the tensor-core kernel takes
+        w, b = self._heads()
+        total = w.shape[2]
+        width = next(c for c in (16, 32, 64, 128) if c >= total)
+        w = torch.cat([w, w.new_zeros((1, w.shape[1], width - total))], dim=2)
+        b = torch.cat([b, b.new_zeros(width - total)])
+        layers.append((core.ConvWeights(w.to(device), bias=b.to(device), relu=False, algo=_lib.ALGO_TC), (1, 1, 0, 0)))
+        return layers
+
+    def _buf(self, n, c, busy, device):
+        pool = self._bufs.setdefault((n, c), [])
+        for t in pool:
+            if t is not busy:
+                return t
+        t = torch.empty((n, c), dtype=torch.float32, device=device)
+        pool.append(t)
+        return t
+
+    def run(self, x, overflow=None):
+        """x: [B, H, W, C] fp32 channels-last BEV features -> list (per task) of dicts like Head.forward (views of one
+        fp32 output buffer).  `overflow` is unused: fp32 activations have no f16 range to leave."""
+        device = x.device
+        b, h, w, c = x.shape
+        with _lib.on_device_of(x):
+            if self._grid is None or (self._grid.batch, self._grid.h, self._grid.w) != (b, h, w):
+                self._grid = BevGrid(b, h, w, device)
+            layers = self._compiled(device)
+            x = x.reshape(b * h * w, c)
+            for cw, geom in layers:
+                rb = self._grid.rulebook(*geom)
+                out = self._buf(self._grid.n_rows, cw.c_out, x, device)
+                core.sparse_conv(x, rb, cw, out)
+                x = out
+        return self._split(x.view(b, h, w, x.shape[1]))
+
+
+def _layer16(conv, bn, relu, extra_pad, device):
+    scale, shift = _folded_bn(bn)
     bias = None if conv.bias is None else conv.bias.detach().float()
     if isinstance(conv, nn.ConvTranspose2d):
         s = int(conv.stride[0])
@@ -257,61 +262,24 @@ def rpn_is_fusable16(rpn):
         return False
 
 
-class FusedBevStack:
-    """RPN + all task heads on NHWC f16 planes (FP16x3, or single-pass FP16 when the input carries one plane: every
+class FusedBevStack(_BevStack):
+    """fp16x3 / fp16: RPN + all task heads on NHWC f16 planes (single-pass FP16 when the input carries one plane: every
     layer then runs on one plane, with the same packed weights): one launch per conv layer, except that each block's run
-    of 3x3 stride-1 layers is one chained launch (conv16.bev_chain), the deblocks write straight into
-    their channel slice of the concat buffer, and the heads of all tasks are ONE 1x1 conv whose fp32 output rows are
-    already the NHWC-permuted layout `Head.forward` produces (mg_head.py:214-230)."""
-
-    def __init__(self, rpn, head):
-        self.rpn, self.head = rpn, head
-        self._sig = None
-        self._plan = None
-        self._bufs = {}
-
-    def _signature(self):
-        ts = [p for p in self.rpn.parameters()] + [b for b in self.rpn.buffers()] + [p for p in self.head.tasks.parameters()]
-        return tuple((t._version, t.data_ptr()) for t in ts)
+    of 3x3 stride-1 layers is one chained launch (conv16.bev_chain), and the deblocks write straight into their channel
+    slice of the concat buffer."""
 
     def _compile(self, device):
         rpn = self.rpn
-        start = rpn._upsample_start_idx
-        blocks = []
-        for blk in rpn.blocks:
-            seq, layers, i, pad = list(blk), [], 0, 0
-            while i < len(seq):
-                m = seq[i]
-                if isinstance(m, nn.ZeroPad2d):
-                    pad = int(m.padding[0])
-                    i += 1
-                elif isinstance(m, nn.Conv2d):
-                    conv, bn, relu, i = _conv_bn_relu(seq, i)
-                    layers.append(_layer16(conv, bn, relu, pad, device))
-                    pad = 0
-                else:
-                    i += 1
-            blocks.append(layers)
+        blocks = [[_layer16(conv, bn, relu, pad, device) for conv, bn, relu, pad in _convs(list(blk))]
+                  for blk in rpn.blocks]
         deblocks = []
         for blk in rpn.deblocks:
-            seq = list(blk)
-            conv, bn, relu, _ = _conv_bn_relu(seq, 0)
+            conv, bn, relu, _ = _conv_bn_relu(list(blk), 0)
             deblocks.append(_layer16(conv, bn, relu, 0, device))
-        # heads: one 1x1 conv over the concatenated output channels of every task
-        ws, bs, self._splits = [], [], []
-        for task in self.head.tasks:
-            parts = [("box_preds", task.conv_box), ("cls_preds", task.conv_cls)]
-            if task.use_dir:
-                parts.append(("dir_cls_preds", task.conv_dir))
-            names = []
-            for name, conv in parts:
-                ws.append(_conv2d_weight(conv))
-                bs.append(conv.bias.detach().float())
-                names.append((name, conv.out_channels))
-            self._splits.append(names)
-        heads = conv16.BevConv16(torch.cat(ws, dim=2), 1, bias=torch.cat(bs), relu=False, device=device)
-        self._plan = dict(blocks=blocks, deblocks=deblocks, heads=heads, start=start,
-                          concat=sum(d.c_out_total for d in deblocks))
+        w, b = self._heads()
+        heads = conv16.BevConv16(w, 1, bias=b, relu=False, device=device)
+        return dict(blocks=blocks, deblocks=deblocks, heads=heads, start=rpn._upsample_start_idx,
+                    concat=sum(d.c_out_total for d in deblocks))
 
     def _planes(self, key, shape, device, n_planes):
         p = self._bufs.get(key)
@@ -338,15 +306,12 @@ class FusedBevStack:
         return out
 
     def run(self, x, overflow=None):
-        """x: Planes [B, H, W, C] -> list (per task) of dicts like Head.forward: box_preds [B,H',W',a*code],
-        cls_preds [B,H',W',a*cls], dir_cls_preds [B,H',W',a*2] (fp32 views of one output buffer)."""
+        """x: Planes [B, H, W, C] -> list (per task) of dicts like Head.forward (fp32 views of one output buffer, on the
+        grid of the deblocks' outputs).  A value that leaves the f16 range ORs 1 into `overflow` (int32[1] device flag,
+        or None)."""
         device = x.device
         with _lib.on_device_of(x.buf):
-            sig = self._signature()
-            if self._plan is None or sig != self._sig:
-                self._compile(device)
-                self._sig = sig
-            pl = self._plan
+            pl = self._compiled(device)
             b, n_planes = x.shape[0], x.n_planes
             concat = None
             col = 0
@@ -384,11 +349,4 @@ class FusedBevStack:
             if out32 is None:
                 out32 = self._bufs[key] = torch.empty((b, hc, wc, heads.c_out_padded), dtype=torch.float32, device=device)
             heads(concat, out_f32=out32, tag="heads")
-        preds, c0 = [], 0
-        for names in self._splits:
-            d = {}
-            for name, c in names:
-                d[name] = out32[..., c0:c0 + c]
-                c0 += c
-            preds.append(d)
-        return preds
+        return self._split(out32)

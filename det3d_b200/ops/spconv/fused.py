@@ -17,16 +17,15 @@ from .modules import SparseConvolution
 
 
 class _Layer:
-    __slots__ = ("conv", "bn", "relu", "residual", "save_identity", "cw", "sig", "cw16", "sig16")
+    __slots__ = ("conv", "bn", "relu", "residual", "save_identity", "cw", "cw16", "sig")
 
     def __init__(self, conv, bn, relu, residual=False, save_identity=False):
         self.conv, self.bn, self.relu = conv, bn, relu
         self.residual = residual            # add the saved block input before the ReLU
         self.save_identity = save_identity  # this layer's INPUT is a block input
-        self.cw = None
-        self.sig = None
-        self.cw16 = None
-        self.sig16 = None
+        self.cw = None      # tf32x3 device weights (core.ConvWeights)
+        self.cw16 = None    # fp16x3 / fp16 device weights (conv16.ConvWeights16)
+        self.sig = {}       # slot name -> the _signature its weights were made from
 
 
 def _bn_fold(bn):
@@ -111,15 +110,21 @@ class FusedSparseEncoder:
         self.overlap_rulebooks = True   # build the rulebook chain on a side stream (see _fork_rulebooks)
 
     # ---- parameters ------------------------------------------------------------
-    def _refresh_weights(self, device):
+    def _refresh_weights(self, slot, device):
+        """Makes each layer's device weights in `slot` ("cw": tf32x3, "cw16": the f16 maths) again where its parameters
+        have changed."""
         for L in self.plan:
-            sig = _signature(L) + (self.algo_override,)
-            if L.cw is not None and L.sig == sig:
+            sig = _signature(L) + ((self.algo_override,) if slot == "cw" else ())
+            if L.sig.get(slot) == sig:
                 continue
             scale, shift = _folded_bn(L, device)
-            L.cw = core.ConvWeights(L.conv.weight.to(device), bias=_conv_bias(L, device), scale=scale, shift=shift,
-                                    relu=L.relu, algo=self.algo_override)
-            L.sig = sig
+            w = L.conv.weight.to(device)
+            kw = dict(bias=_conv_bias(L, device), scale=scale, shift=shift, relu=L.relu)
+            if slot == "cw":
+                L.cw = core.ConvWeights(w, algo=self.algo_override, **kw)
+            else:
+                L.cw16 = conv16.ConvWeights16(w, **kw)
+            L.sig[slot] = sig
 
     # ---- buffers -----------------------------------------------------------------
     def _build_state(self, cap0, spatial, batch, device):
@@ -227,7 +232,9 @@ class FusedSparseEncoder:
             return self._run(features, coors, batch_size, spatial, n_dev, row_cap, bev_rows)
 
     def _run(self, features, coors, batch_size, spatial, n_dev=None, row_cap=None, bev_rows=False):
-        """features [M, C] f32, coors [M, 4] int (b,z,y,x) -> dense [B, C_out, D, H, W].
+        """features [M, C] f32, coors [M, 4] int (b,z,y,x) -> dense [B, C_out, D, H, W]; with `bev_rows` fp32 BEV rows
+        [B*H*W, C*D] (channel = c*D + z: the values of dense.view(B, C*D, H, W), channels last), with
+        bev_rows="planes" (f16 maths only) NHWC planes [B, H, W, C*D].
 
         With `n_dev` (int32[>=1] device tensor) only the first n_dev[0] rows are
         live and M is a capacity; otherwise all M rows are live.
@@ -239,53 +246,90 @@ class FusedSparseEncoder:
         if (st is None or st["cap0"] < cap_needed or st["batch"] != batch_size
                 or st["spatial"] != tuple(spatial) or st["device"] != device):
             st = self._state = self._build_state(cap_needed, spatial, batch_size, device)
-        if self.math in ("fp16x3", "fp16") and self.algo_override is None:
-            return self._run16(st, features, coors, batch_size, n_dev, bev_rows)
-        if bev_rows == "planes":
+        f16 = self.math in ("fp16x3", "fp16") and self.algo_override is None
+        if bev_rows == "planes" and not f16:
             raise ValueError("BEV planes are produced by the fp16x3 / fp16 paths only")
-        self._refresh_weights(device)
-        x = self._adopt_level0(st, features, coors, n_dev).contiguous()
-        _side, before_conv = self._fork_rulebooks(st, device)
+        slot = "cw16" if f16 else "cw"
+        self._refresh_weights(slot, device)
+        feats = self._adopt_level0(st, features, coors, n_dev)
+        if f16:
+            ovf = self.external_overflow
+            if ovf is None:
+                ovf = st.get("overflow")
+                if ovf is None:
+                    ovf = st["overflow"] = torch.zeros(1, dtype=torch.int32, device=device)
+            n_planes = self.n_planes
+            pool = ("p16", n_planes)
+            make = lambda cap, c: conv16.Planes((max(cap, 1), c), device, n_planes=n_planes)
+            conv = lambda x, rb, cw, out, residual: conv16.sparse_conv16(x, rb, cw, out, residual=residual,
+                                                                         overflow=ovf)
+        else:
+            pool = ("f32",)
+            make = lambda cap, c: torch.empty((max(cap, 1), c), dtype=torch.float32, device=device)
+            conv = core.sparse_conv
+        side, before_conv = self._fork_rulebooks(st, device)
+        planes_cleared = None
+        if f16 and bev_rows and side is not None:
+            # the BEV planes are cleared behind the rulebook chain, off the critical path (18 MB for SECOND)
+            with torch.cuda.stream(side):
+                self._bev_planes(st, batch_size, device).zero_()
+                planes_cleared = torch.cuda.Event()
+                planes_cleared.record(side)
+
+        if not f16:
+            x = feats.contiguous()
+        elif self.plan[0].cw16.fp32_input:
+            x = feats
+        else:
+            x = conv16.Planes.from_f32(feats, ovf, n_planes=n_planes)
         identity = None
         for L, rb, build in st["steps"]:
             before_conv(rb, build)
             if L.save_identity:
                 identity = x
             cap, c = rb.out_level.cap, L.conv.out_channels
-            out = self._take(st["pools"], (cap, c), (x, identity),
-                             lambda: torch.empty((max(cap, 1), c), dtype=torch.float32, device=device))
-            core.sparse_conv(x, rb, L.cw, out, residual=identity if L.residual else None)
+            out = self._take(st["pools"], pool + (cap, c), (x, identity), lambda: make(cap, c))
+            conv(x, rb, getattr(L, slot), out, residual=identity if L.residual else None)
             if L.residual:
                 identity = None
             x = out
-        if bev_rows:
-            # channels-last [B*H*W, C*D] with channel = c*D + z: same values as dense.view(B, C*D, H, W)
-            d, h, w = st["final_level"].spatial
-            rows = st.get("bev_rows")
-            if rows is None:
-                rows = st["bev_rows"] = torch.empty((batch_size * h * w, x.shape[1] * d), dtype=torch.float32, device=device)
+
+        final = st["final_level"]
+        d, h, w = final.spatial
+        c = x.shape[-1]
+        rows_shape = (batch_size * h * w, c * d)
+        if bev_rows and not f16:
+            rows = self._f32_buffer(st, "bev_rows", rows_shape, device)
             rows.zero_()
-            core.sparse_to_bev_rows(x, st["final_level"], rows)
-            return rows
+            return core.sparse_to_bev_rows(x, final, rows)
+        if bev_rows:
+            planes = self._bev_planes(st, batch_size, device)
+            assert tuple(planes.shape) == (batch_size, h, w, c * d)
+            if planes_cleared is not None:
+                torch.cuda.current_stream(device).wait_event(planes_cleared)
+            else:
+                planes.zero_()
+            conv16.sparse_to_bev16(x, final, planes)
+            if bev_rows == "planes":
+                return planes
+            return planes.view(*rows_shape).to_f32(out=self._f32_buffer(st, "bev_rows", rows_shape, device))
+        if f16:
+            x = x.to_f32(out=self._f32_buffer(st, "final_f32", (max(final.cap, 1), c), device))
         dense = st["dense"]
         dense.zero_()
-        core.sparse_to_dense(x, st["final_level"], out=dense)
-        return dense
+        return core.sparse_to_dense(x, final, out=dense)
 
-    # ---- FP16x3 / single-pass FP16 path ---------------------------------------------------------
+    @staticmethod
+    def _f32_buffer(st, key, shape, device):
+        """The state's fp32 buffer `key`, allocated on first use."""
+        t = st.get(key)
+        if t is None:
+            t = st[key] = torch.empty(shape, dtype=torch.float32, device=device)
+        return t
+
     @property
     def n_planes(self):
         return 1 if self.math == "fp16" else 2
-
-    def _refresh_weights16(self, device):
-        for L in self.plan:
-            sig = _signature(L)
-            if L.cw16 is not None and L.sig16 == sig:
-                continue
-            scale, shift = _folded_bn(L, device)
-            L.cw16 = conv16.ConvWeights16(L.conv.weight.to(device), bias=_conv_bias(L, device), scale=scale, shift=shift,
-                                          relu=L.relu)
-            L.sig16 = sig
 
     def _bev_planes(self, st, batch_size, device):
         """NHWC f16 planes [B, H, W, C * D] of the encoder output (scn.py:192-195: dense.view(N, C * D, H, W))."""
@@ -307,65 +351,6 @@ class FusedSparseEncoder:
         if hit:
             flag.zero_()
         return hit
-
-    def _run16(self, st, features, coors, batch_size, n_dev, bev_rows):
-        device = features.device
-        self._refresh_weights16(device)
-        feats = self._adopt_level0(st, features, coors, n_dev)
-        ovf = self.external_overflow
-        if ovf is None:
-            ovf = st.get("overflow")
-            if ovf is None:
-                ovf = st["overflow"] = torch.zeros(1, dtype=torch.int32, device=device)
-        side, before_conv = self._fork_rulebooks(st, device)
-        planes_cleared = None
-        if bev_rows and side is not None:
-            # the BEV planes are cleared behind the rulebook chain, off the critical path (18 MB for SECOND)
-            with torch.cuda.stream(side):
-                self._bev_planes(st, batch_size, device).zero_()
-                planes_cleared = torch.cuda.Event()
-                planes_cleared.record(side)
-
-        first = self.plan[0].cw16
-        n_planes = self.n_planes
-        x = feats if first.fp32_input else conv16.Planes.from_f32(feats, ovf, n_planes=n_planes)
-        identity = None
-        for L, rb, build in st["steps"]:
-            before_conv(rb, build)
-            if L.save_identity:
-                identity = x
-            cap, c = rb.out_level.cap, L.conv.out_channels
-            out = self._take(st["pools"], ("p16", n_planes, cap, c), (x, identity),
-                             lambda: conv16.Planes((max(cap, 1), c), device, n_planes=n_planes))
-            conv16.sparse_conv16(x, rb, L.cw16, out, residual=identity if L.residual else None, overflow=ovf)
-            if L.residual:
-                identity = None
-            x = out
-        final = st["final_level"]
-        d, h, w = final.spatial
-        c = x.shape[-1]
-        if bev_rows:
-            planes = self._bev_planes(st, batch_size, device)
-            assert tuple(planes.shape) == (batch_size, h, w, c * d)
-            if planes_cleared is not None:
-                torch.cuda.current_stream(device).wait_event(planes_cleared)
-            else:
-                planes.zero_()
-            conv16.sparse_to_bev16(x, final, planes)
-            if bev_rows == "planes":
-                return planes
-            rows = st.get("bev_rows")
-            if rows is None:
-                rows = st["bev_rows"] = torch.empty((batch_size * h * w, c * d), dtype=torch.float32, device=device)
-            return planes.view(batch_size * h * w, c * d).to_f32(out=rows)
-        rows32 = st.get("final_f32")
-        if rows32 is None:
-            rows32 = st["final_f32"] = torch.empty((max(final.cap, 1), c), dtype=torch.float32, device=device)
-        x.to_f32(out=rows32)
-        dense = st["dense"]
-        dense.zero_()
-        core.sparse_to_dense(rows32, final, out=dense)
-        return dense
 
     def accounting(self):
         """Algorithmic bytes / flops of the most recent run (SURVEY 8d formulas; synchronises).
