@@ -128,6 +128,7 @@ SIGNATURES = {
     "d3b_frustum_crop_workspace_bytes": (_sz, [_i32, _i32]),
     "d3b_frustum_crop_dev": (C.c_int, [_vp, _i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
     "d3b_kitti_results_dev": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "d3b_nusc_results_dev": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp]),
     "d3b_rulebook_workspace_bytes": (_sz, [_i64]),
     "d3b_index_build_hash": (C.c_int, [_vp, _vp, _i32, C.POINTER(SiteIndex), _vp]),
     "d3b_rulebook_subm": (C.c_int, [_vp, _vp, _i32, C.POINTER(SiteIndex), _I3, _vp, _vp, _vp]),

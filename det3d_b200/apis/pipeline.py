@@ -25,6 +25,8 @@ from det3d_b200.datasets.pipelines.loading import (MAX_BATCH, MAX_SWEEPS, Batche
 from det3d_b200.models import build_detector
 from det3d_b200.ops.point_cloud.frustum import MAX_NDIM, MIN_NDIM, FrustumCrop
 from det3d_b200.ops.point_cloud.kitti_results import KittiResults, calib_table, check_calibs, to_annos
+from det3d_b200.ops.point_cloud.nusc_results import (ND as NUSC_ND, NuscResults, attribute_table, check_tokens,
+                                                     pose_table, to_nusc_annos)
 from det3d_b200.ops.point_cloud.voxelize import Voxelizer
 
 
@@ -55,12 +57,14 @@ class InferencePipeline:
         # _GraphEntry by key, least recently used first: (batch, bucket, ndim) (forward_graphed, infer_host), (batch,
         # raw bucket, table capacity, raw_stride, n_feat) (infer_sweeps), ("stream", B, K, slot_capacity, raw_stride,
         # n_feat) (SweepStream.infer), ("frustum", B, raw bucket, ndim) / ("frustum_kitti", B, raw bucket, ndim)
-        # (infer_raw without / with kitti_results)
+        # (infer_raw without / with kitti_results); ("sweeps_nusc",) + infer_sweeps' key and the stream's key + ("nusc",)
+        # (nusc_results=True)
         self._graphs = collections.OrderedDict()
         self.max_graphs = 8
         self._ovf_host = None
         self._planes = collections.OrderedDict()      # calibration bytes -> frustum planes f64 [6, 4] (infer_raw)
         self._kitti_tables = collections.OrderedDict()   # calibration bytes -> KITTI results table f64 [32]
+        self._nusc_tables = collections.OrderedDict()    # pose record bytes -> nuScenes pose table f64 [32]
 
     def anchors(self, batch):
         a = self._anchor_cache.get(batch)
@@ -277,7 +281,8 @@ class InferencePipeline:
         return self._serve(graphed, key, make, step, self._packed_into(pinned_out), stage)
 
     @torch.no_grad()
-    def infer_sweeps(self, samples, pinned_out=None, graphed=False, n_feat=4, radius=1.0):
+    def infer_sweeps(self, samples, pinned_out=None, graphed=False, n_feat=4, radius=1.0, nusc_results=False, poses=None,
+                     tokens=None):
         """Multi-sweep samples -> host detections [B, D, nd+3], as infer_host.
 
         samples: [(raw_sweeps, transforms, time_lags), ...], one per cloud, each with ingest_sweeps' contract (raw
@@ -288,7 +293,19 @@ class InferencePipeline:
         forward per (B, raw bucket, sweep-table capacity, raw_stride, n_feat) (bucket_of of the raw total); the raw
         sweeps are copied into its static raw buffer and the sweep table is copied H2D only when it changed.  Raises
         ValueError before anything is enqueued when the samples are malformed or n_feat + 1 is not the reader's
-        feature count.  The overflow fallback is infer_host's."""
+        feature count.  The overflow fallback is infer_host's.
+
+        nusc_results=True returns instead what the reference reports for nuScenes (NuScenesDataset.evaluation,
+        det3d/datasets/nuscenes/nuscenes.py:180-274): the nusc_annos dict, results keyed by tokens[b] in sample order,
+        each detection in predict's order as a submission box in the global frame -- translation, size, orientation
+        quaternion, velocity, class name (self.class_names()), score and attribute -- and the reference's meta.
+        poses[b] holds sample b's key-frame records dict(calibrated_sensor=dict(translation, rotation),
+        ego_pose=dict(translation, rotation)) and tokens[b] its sample token.  d3b_nusc_results_dev runs right after
+        predict, inside the same graph when graphed (keyed ("sweeps_nusc",) + the plain key); the pose table
+        (nusc_pose_table, cached per record) goes H2D only when it differs from that graph's last replay, and the rows,
+        their counts and the f16-range flag come back before one sync.  ValueError before anything is enqueued when
+        poses or tokens are missing or not one per sample, a token is not a str or repeats, a record is malformed, a
+        class has no nuScenes attribute, or the model's boxes have no velocity (nd != 9)."""
         if n_feat + 1 != self.num_point_features:
             raise ValueError("ingested clouds have n_feat + 1 = %d features, the reader takes %d"
                              % (n_feat + 1, self.num_point_features))
@@ -296,17 +313,28 @@ class InferencePipeline:
         stride, sizes = check_sweep_samples(samples, n_feat)
         batch, total = len(samples), sum(map(sum, sizes))
         key = (batch, self.bucket_of(total), sweep_table_capacity(sum(map(len, sizes)), batch), stride, n_feat)
+        nusc = _NuscStep(self, batch, poses, tokens) if nusc_results else None
 
         def make():
             # eager too, the voxelizer's capacity is the bucket: it keeps its device-offset buffers per capacity
             ingest = BatchedIngest(*key, radius, self.device)
-            return _GraphEntry(ingest=ingest, table=_Upload(ingest.table), rows=RowStager())
+            entry = _GraphEntry(ingest=ingest, table=_Upload(ingest.table), rows=RowStager())
+            return entry if nusc is None else nusc.attach(entry)
 
         def stage(e):
             e.table.put(e.ingest.host_table(samples, sizes))
             e.rows.put([r for raws, _tms, _lags in samples for r in raws], e.ingest.raw)
-        return self._serve(graphed, key, make, lambda e: self.pack(self.forward_device(*e.ingest.launch())),
-                           self._packed_into(pinned_out), stage, fits=lambda e: e.ingest.radius == radius)
+            if nusc is not None:
+                nusc.stage(e)
+
+        def step(e):
+            packed = self.pack(self.forward_device(*e.ingest.launch()))
+            return packed if nusc is None else e.nusc.launch(packed)
+        if nusc is None:
+            return self._serve(graphed, key, make, step, self._packed_into(pinned_out), stage,
+                               fits=lambda e: e.ingest.radius == radius)
+        return nusc.annos(self._serve(graphed, ("sweeps_nusc",) + key, make, step, _NuscStep.fetch, stage,
+                                      fits=lambda e: e.ingest.radius == radius))
 
     # ---- raw KITTI scans: camera-frustum crop on the device ----------------------------------------------------------
     @staticmethod
@@ -365,6 +393,25 @@ class InferencePipeline:
         by numpy's matmul, P2, the image shape), cached by the calibration's bytes."""
         return self._cached_per_calib(self._kitti_tables, calib,
                                       lambda c, shape: calib_table(dict(c, image_shape=shape)))
+
+    def nusc_pose_table(self, record):
+        """The nuScenes results kernel's pose row f64 [32] of one sample's records (ops.point_cloud.nusc_results.
+        pose_table), cached by the records' bytes (the sensor calibration is fixed per scene and the ego pose changes per
+        sample), the 256 most recently used kept.  ValueError for a malformed record."""
+        try:
+            parts = [np.ascontiguousarray(record[k][f], np.float64) for k in ("calibrated_sensor", "ego_pose")
+                     for f in ("translation", "rotation")]
+        except (KeyError, TypeError, ValueError):
+            return pose_table(record)                   # raises the record's ValueError
+        key = b"".join(p.tobytes() for p in parts) + repr([p.shape for p in parts]).encode()
+        value = self._nusc_tables.get(key)
+        if value is None:
+            value = self._nusc_tables[key] = pose_table(record)
+            while len(self._nusc_tables) > 256:
+                self._nusc_tables.popitem(last=False)
+        else:
+            self._nusc_tables.move_to_end(key)
+        return value
 
     def class_names(self):
         """The config's class names flattened over its tasks, the order predict's labels index."""
@@ -439,6 +486,45 @@ class InferencePipeline:
             m = row[:, -1] > 0.5
             out.append(dict(box3d_lidar=row[m, :-3], scores=row[m, -3], label_preds=row[m, -2].long()))
         return out
+
+
+class _NuscStep:
+    """infer_sweeps' and SweepStream.infer's nuScenes results post-step.  The constructor checks the arguments and
+    builds the pose tables (ValueError before anything is enqueued); attach adds a NuscResults and its pose _Upload to a
+    new entry, stage uploads the poses when they changed, fetch enqueues the D2H of the rows, annos formats them."""
+
+    def __init__(self, pipe, batch, poses, tokens):
+        if poses is None or tokens is None:
+            raise ValueError("nusc_results needs poses and tokens, one per sample")
+        poses = list(poses)
+        if len(poses) != batch:
+            raise ValueError("%d samples but %d pose records" % (batch, len(poses)))
+        self.tokens = check_tokens(tokens, batch)
+        nd = pipe.model.bbox_head.box_coder.n_dim            # the decoded box (code_size adds the sin / cos pair)
+        if nd != NUSC_ND:
+            raise ValueError("nuScenes results need boxes with velocity (nd = %d), the model's have nd = %d"
+                             % (NUSC_ND, nd))
+        self.class_names = pipe.class_names()
+        self.table = attribute_table(self.class_names)
+        self.poses = np.stack([pipe.nusc_pose_table(p) for p in poses])
+        self.batch, self.device = batch, pipe.device
+
+    def attach(self, entry):
+        entry.nusc = NuscResults(self.batch, self.device)
+        entry.poses = _Upload(entry.nusc.poses)
+        entry.pose_uploads = 0                        # H2D copies of the pose table so far
+        return entry
+
+    def stage(self, entry):
+        entry.pose_uploads += entry.poses.put(self.poses)
+
+    @staticmethod
+    def fetch(entry, _out):
+        return entry.nusc.fetch()
+
+    def annos(self, nusc):
+        return to_nusc_annos(nusc.results_host.numpy(), nusc.counts_host.numpy(), self.class_names, self.tokens,
+                             self.table)
 
 
 class _GraphEntry:
@@ -586,13 +672,24 @@ class SweepStream:
         self.pending_h2d_bytes = 0
 
     @torch.no_grad()
-    def infer(self, pinned_out=None, graphed=False):
+    def infer(self, pinned_out=None, graphed=False, nusc_results=False, poses=None, tokens=None):
         """Detections of the current frame, host [B, D, nd+3] as infer_sweeps returns them, and bit-identical to
         infer_sweeps(samples()).  The only H2D is the sweep table (the sweeps went with push).  graphed=True replays the
         stream's CUDA graph.  On an f16-range overflow the model switches to tf32x3 and the same frame is re-run, as in
-        infer_sweeps; the history is not touched.  ValueError when a stream holds no sweep."""
-        self._stage_table()
+        infer_sweeps; the history is not touched.  ValueError when a stream holds no sweep.
+
+        nusc_results=True (with poses and tokens, one per stream) returns the frame's nusc_annos as
+        infer_sweeps(samples(), nusc_results=True) does, from the stream's graph keyed key + ("nusc",); the pose table
+        goes H2D only when it changed."""
         pipe = self.pipe
-        return pipe._serve(graphed, self.key, lambda: _GraphEntry(stream=self),
-                           lambda e: pipe.pack(pipe.forward_device(*self._ingest.launch())),
-                           pipe._packed_into(pinned_out), fits=lambda e: e.stream is self)
+        nusc = _NuscStep(pipe, self.batch, poses, tokens) if nusc_results else None
+        self._stage_table()
+
+        def step(e):
+            packed = pipe.pack(pipe.forward_device(*self._ingest.launch()))
+            return packed if nusc is None else e.nusc.launch(packed)
+        if nusc is None:
+            return pipe._serve(graphed, self.key, lambda: _GraphEntry(stream=self), step, pipe._packed_into(pinned_out),
+                               fits=lambda e: e.stream is self)
+        return nusc.annos(pipe._serve(graphed, self.key + ("nusc",), lambda: nusc.attach(_GraphEntry(stream=self)),
+                                      step, _NuscStep.fetch, nusc.stage, fits=lambda e: e.stream is self))

@@ -21,9 +21,10 @@
 // __f*_rn, so nothing is contracted into an FMA; sin / cos / atan2 are the CUDA math library's.  The SASS's DFMA / FFMA
 // come only from those and from the correctly rounded division sequences.
 //
-// One CTA per sample walks its D rows in chunks of kKrThreads and compacts the kept rows in order (ballot + block
-// scan); rows past the sample's count are written as zeros.  No workspace.
+// One CTA per sample walks its D rows in chunks of kKrThreads and compacts the kept rows in order (compact_rows.cuh);
+// rows past the sample's count are written as zeros.  No workspace.
 #include "common.cuh"
+#include "compact_rows.cuh"
 
 namespace d3b {
 namespace {
@@ -106,40 +107,16 @@ kitti_results_kernel(const float* __restrict__ det, const double* __restrict__ c
                      double* __restrict__ results, int* __restrict__ counts) {
   __shared__ double cal[kKrCalibDoubles];
   __shared__ int warp_cnt[kKrThreads / 32];
-  const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int b = blockIdx.x;
   if (threadIdx.x < kKrCalibDoubles) cal[threadIdx.x] = calib[(size_t)b * kKrCalibDoubles + threadIdx.x];
   __syncthreads();
   const int stride = nd + 3;
   const float* __restrict__ det_b = det + (size_t)b * D * stride;
-  double* __restrict__ out_b = results + (size_t)b * D * kKrCols;
-  int count = 0;                                    // kept rows so far, the same in every thread
-  for (int base = 0; base < D; base += kKrThreads) {
-    const int i = base + threadIdx.x;
-    double row[kKrCols];
-    bool keep = false;
-    if (i < D) {
-      const float* d = det_b + (size_t)i * stride;
-      keep = d[nd + 2] > 0.5f && kitti_row(d, nd, cal, row);
-    }
-    const unsigned bal = __ballot_sync(0xffffffffu, keep);
-    if (lane == 0) warp_cnt[warp] = __popc(bal);
-    __syncthreads();
-    int before = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < kKrThreads / 32; ++w) {
-      const int n = warp_cnt[w];
-      before += w < warp ? n : 0;
-      total += n;
-    }
-    if (keep) {
-      double* o = out_b + (size_t)(count + before + __popc(bal & ((1u << lane) - 1u))) * kKrCols;
-#pragma unroll
-      for (int j = 0; j < kKrCols; ++j) o[j] = row[j];
-    }
-    count += total;
-    __syncthreads();                                // warp_cnt is rewritten by the next chunk
-  }
-  for (size_t j = (size_t)count * kKrCols + threadIdx.x; j < (size_t)D * kKrCols; j += kKrThreads) out_b[j] = 0.0;
+  const int count = compact_rows<kKrThreads, kKrCols>(D, results + (size_t)b * D * kKrCols, warp_cnt,
+                                                      [&](int i, double* row) {
+    const float* d = det_b + (size_t)i * stride;
+    return d[nd + 2] > 0.5f && kitti_row(d, nd, cal, row);
+  });
   if (threadIdx.x == 0) counts[b] = count;
 }
 

@@ -193,6 +193,25 @@ int d3b_frustum_crop_dev(const float* points, int32_t point_capacity, int32_t nd
 int d3b_kitti_results_dev(const float* detections, const double* calib, int32_t batch, int32_t max_det, int32_t nd,
                           double* results, int32_t* counts, void* stream);
 
+/* nuScenes result rows from predict's packed detections, for graph replay.  replaces the per-box loop of
+ * NuScenesDataset.evaluation (det3d/datasets/nuscenes/nuscenes.py:219-259) with _second_det_to_nusc_box and
+ * _lidar_nusc_box_to_global (det3d/datasets/nuscenes/nusc_common.py:222-265): yaw' = -r - pi/2 in f32, the orientation
+ * quaternion about z, then the sensor -> ego -> global rotation and translation of the centre, the velocity and the
+ * orientation in f64, and the reference's speed test (> 0.2 m/s in f64) that picks the attribute.
+ * 1 <= batch <= 64, 0 <= max_det <= 2^20, nd 9 (x, y, z, w, l, h, vx, vy, r; D3B_ERR_UNSUPPORTED otherwise).
+ * detections [batch][max_det][12] f32 device: box, score, label, valid (a row counts when valid > 0.5)
+ * poses      [batch][32] f64 DEVICE: the key frame's calibrated_sensor rotation matrix Rc (row-major) [0, 9) and
+ *            translation tc [9, 12), its ego_pose rotation matrix Rp [12, 21) and translation tp [21, 24), the two
+ *            rotations as unit quaternions (w, x, y, z) qc [24, 28) and qp [28, 32)
+ * results    [batch][max_det][15] f64 device: per valid detection, in predict's order, translation 3 (global), size 3
+ *            (w, l, h), rotation 4 (w, x, y, z), velocity 2 (global x, y), score, label, moving (1 or 0); rows at or
+ *            past counts[b] are written as zeros
+ * counts     [batch] i32 device: valid detections of each sample
+ * Every f64 product and sum is rounded on its own in a fixed order (no FMA contraction); sin / cos are the CUDA math
+ * library's.  One kernel, one CTA per sample, no host sync, no workspace. */
+int d3b_nusc_results_dev(const float* detections, const double* poses, int32_t batch, int32_t max_det, int32_t nd,
+                         double* results, int32_t* counts, void* stream);
+
 /* ========================================================================= *
  * 2. Rulebook (sparse-convolution index maps)
  *    replaces spconv v1.x `get_indice_pairs` as called by SubMConv3d /
