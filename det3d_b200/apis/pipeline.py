@@ -31,6 +31,8 @@ from det3d_b200.ops.point_cloud.voxelize import Voxelizer
 
 
 class InferencePipeline:
+    _pending = ()                                     # (a pipeline made without __init__ has no unfinished frame)
+
     def __init__(self, cfg, model=None, device="cuda", strict_fp32=True):
         self.cfg = cfg
         self.device = torch.device(device)
@@ -56,12 +58,14 @@ class InferencePipeline:
         self.strict_fp32 = strict_fp32
         # _GraphEntry by key, least recently used first: (batch, bucket, ndim) (forward_graphed, infer_host), (batch,
         # raw bucket, table capacity, raw_stride, n_feat) (infer_sweeps), ("stream", B, K, slot_capacity, raw_stride,
-        # n_feat) (SweepStream.infer), ("frustum", B, raw bucket, ndim) / ("frustum_kitti", B, raw bucket, ndim)
+        # n_feat[, ("in_flight", k)]) (SweepStream.infer), ("frustum", B, raw bucket, ndim) / ("frustum_kitti", B, raw bucket, ndim)
         # (infer_raw without / with kitti_results); ("sweeps_nusc",) + infer_sweeps' key and the stream's key + ("nusc",)
         # (nusc_results=True)
         self._graphs = collections.OrderedDict()
         self.max_graphs = 8
-        self._ovf_host = None
+        self.max_in_flight = 2                        # unfinished frames; a submit beyond the bound completes the oldest
+        self._pending = collections.deque()           # unfinished frames (PendingResult), in submission order
+        self._pinned_free = collections.defaultdict(list)   # (shape, dtype) -> pinned host outputs no frame holds
         self._planes = collections.OrderedDict()      # calibration bytes -> frustum planes f64 [6, 4] (infer_raw)
         self._kitti_tables = collections.OrderedDict()   # calibration bytes -> KITTI results table f64 [32]
         self._nusc_tables = collections.OrderedDict()    # pose record bytes -> nuScenes pose table f64 [32]
@@ -109,7 +113,8 @@ class InferencePipeline:
     def set_math(self, math):
         """Switch the model's convolutions to `math` ("fp16x3", the default; "fp16", single-pass FP16; or "tf32x3") and
         drop the captured graphs: a graph replays the kernels it was captured with, so one captured under another math
-        would keep running that math."""
+        would keep running that math.  Unfinished frames are completed first, on the math they were submitted under."""
+        self.drain()
         self.model.set_math(math)
         self._graphs.clear()
 
@@ -158,42 +163,94 @@ class InferencePipeline:
         entry = self._graphs[key] = make()
         return entry
 
-    def _serve(self, graphed, key, make, step, fetch, stage=None, fits=None):
-        """Runs one entry point: takes its entry (graphed: _cached(key, make, fits); eager: a transient make()), stages
-        the inputs into it (stage(entry)), runs step(entry) -- eagerly, or captured into and replayed from entry.graph
-        -- enqueues the D2H copies of fetch(entry, step's outputs), and syncs once.  When the f16-range flag was raised,
-        the model has switched to tf32x3 and check_overflow has dropped the graphs, so everything runs once more from
-        a fresh lookup.  Returns fetch's host result."""
-        for _attempt in range(2):
+    def _serve(self, graphed, key, make, step, fetch, stage=None, fits=None, finish=None, block=True, hold=None):
+        """Runs one frame of an entry point: takes its entry (graphed: _cached(key, make, fits); eager: a transient
+        make()), stages the inputs into it (stage(entry)), runs step(entry) -- eagerly, or captured into and replayed
+        from entry.graph -- enqueues the D2H copies of fetch(entry, step's outputs, frame) and of the f16-range flag
+        into the frame's own pinned int, and clears the flag, so a raised flag names its frame.  Everything is on the
+        current stream, in submission order.  First, while max_in_flight frames are unfinished, the oldest is completed.
+
+        Returns the frame's PendingResult (block=False) or its result (block=True, one sync): finish(fetch's host
+        value), or that value itself.  hold(), called right before the frame is enqueued, returns what to call once it
+        is complete (SweepStream's slots).  Completing a frame whose flag was raised switches to tf32x3 (check_overflow)
+        and re-runs it and every later unfinished frame, in submission order, from a fresh lookup -- which is what a
+        sequence of blocking calls computes."""
+        def run(frame):
             entry = self._cached(key, make, fits) if graphed else make()
             if stage is not None:
                 stage(entry)
             out = self._run_graph(entry, lambda: step(entry)) if graphed else step(entry)
-            host = fetch(entry, out)
-            if not self._sync_overflow():
-                break
-        return host
+            host = fetch(entry, out, frame)
+            flag = self.overflow_flag()
+            if flag is not None:
+                frame.pinned("overflow", flag).copy_(flag, non_blocking=True)
+                flag.zero_()
+            return entry, host
+        while self._pending and len(self._pending) >= self.max_in_flight:
+            self._complete_oldest()
+        release = None if hold is None else hold()
+        frame = PendingResult(self, run, finish, release)
+        try:
+            frame._launch()
+        except BaseException:
+            if release is not None:
+                release()
+            raise
+        self._pending.append(frame)
+        return frame.result() if block else frame
+
+    def _complete_oldest(self):
+        """Waits for the oldest unfinished frame and hands it its result.  On a raised f16-range flag: check_overflow,
+        then every unfinished frame -- this one first -- runs once more (a re-run that overflows again only warns)."""
+        frame = self._pending[0]
+        frame._event.synchronize()
+        flag = frame._bufs.get("overflow")
+        if flag is not None and int(flag[0]):
+            rerun = not frame.rerun
+            if rerun:
+                self._pending[-1]._event.synchronize()      # none of them still runs when check_overflow drops graphs
+            self.check_overflow(1)
+            if rerun:
+                for f in self._pending:
+                    f.rerun = True
+                    f._launch()
+                frame._event.synchronize()
+                flag = frame._bufs.get("overflow")
+                if flag is not None and int(flag[0]):
+                    self.check_overflow(1)
+        self._pending.popleft()
+        frame._finish_now()
+
+    def drain(self):
+        """Completes every unfinished frame (their handles keep the results)."""
+        while self._pending:
+            self._complete_oldest()
+
+    def _pinned_take(self, shape, dtype):
+        free = self._pinned_free[(tuple(shape), dtype)]
+        return free.pop() if free else torch.empty(shape, dtype=dtype, pin_memory=True)
+
+    def _pinned_give(self, buf):
+        self._pinned_free[(tuple(buf.shape), buf.dtype)].append(buf)
 
     @staticmethod
     def _packed_into(pinned_out):
-        """_serve's fetch of the packed detections: their D2H copy into pinned_out (allocated pinned when None)."""
-        def fetch(_entry, packed):
+        """_serve's fetch of the packed detections: their D2H copy into pinned_out (allocated pinned when None; a
+        re-run copies into the same buffer)."""
+        def fetch(_entry, packed, _frame):
             nonlocal pinned_out
             if pinned_out is None:
                 pinned_out = torch.empty(packed.shape, dtype=torch.float32, pin_memory=True)
             return pinned_out.copy_(packed, non_blocking=True)
         return fetch
 
-    def _sync_overflow(self):
-        """D2H of the f16-range flag behind the copies already enqueued, then one sync.  Returns True when the flag was
-        raised and the model has switched to tf32x3 (check_overflow)."""
-        flag = self.overflow_flag()
-        if flag is not None:
-            if self._ovf_host is None:
-                self._ovf_host = torch.zeros(1, dtype=torch.int32, pin_memory=True)
-            self._ovf_host.copy_(flag, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        return flag is not None and self.check_overflow(int(self._ovf_host[0]))
+    @staticmethod
+    def _rows_into(_entry, out, frame):
+        """_serve's fetch of a results post-step: the D2H copies of its (results, counts) into the frame's own pinned
+        buffers."""
+        results, counts = out
+        return (frame.pinned("results", results).copy_(results, non_blocking=True),
+                frame.pinned("counts", counts).copy_(counts, non_blocking=True))
 
     def _points_entry(self, batch, bucket, ndim):
         """forward_graphed's entry (batch, bucket, ndim): static points [bucket, ndim] and device offsets [batch + 1]."""
@@ -254,11 +311,16 @@ class InferencePipeline:
                           det["valid"].float().unsqueeze(-1)], dim=-1).contiguous()
 
     @torch.no_grad()
-    def infer_host(self, clouds, pinned_out=None, graphed=False):
+    def infer_host(self, clouds, pinned_out=None, graphed=False, block=True):
         """clouds: list of pinned (or plain) host float32 tensors [N_i, ndim].
         H2D copy, forward, D2H of the packed detections.  Returns a host tensor [B, D, nd+3].
         graphed=True copies the clouds into the static input of the (batch, bucket) graph and replays it
-        (forward_graphed); the detections are the same bits."""
+        (forward_graphed); the detections are the same bits.
+
+        block=False returns a PendingResult once the frame is enqueued, without a sync; its result() is what the
+        blocking call returns.  As every entry point's block=False, the inputs (and pinned_out) are kept for a possible
+        re-run on tf32x3 and must stay unchanged until result(); pinned tensors are also copied to the device from
+        where they are."""
         offsets = [0]
         for c in clouds:
             offsets.append(offsets[-1] + c.shape[0])
@@ -278,11 +340,11 @@ class InferencePipeline:
             e.rows.put(clouds, e.points)
             if graphed:
                 e.offsets.put(offsets)
-        return self._serve(graphed, key, make, step, self._packed_into(pinned_out), stage)
+        return self._serve(graphed, key, make, step, self._packed_into(pinned_out), stage, block=block)
 
     @torch.no_grad()
     def infer_sweeps(self, samples, pinned_out=None, graphed=False, n_feat=4, radius=1.0, nusc_results=False, poses=None,
-                     tokens=None):
+                     tokens=None, block=True):
         """Multi-sweep samples -> host detections [B, D, nd+3], as infer_host.
 
         samples: [(raw_sweeps, transforms, time_lags), ...], one per cloud, each with ingest_sweeps' contract (raw
@@ -305,7 +367,9 @@ class InferencePipeline:
         (nusc_pose_table, cached per record) goes H2D only when it differs from that graph's last replay, and the rows,
         their counts and the f16-range flag come back before one sync.  ValueError before anything is enqueued when
         poses or tokens are missing or not one per sample, a token is not a str or repeats, a record is malformed, a
-        class has no nuScenes attribute, or the model's boxes have no velocity (nd != 9)."""
+        class has no nuScenes attribute, or the model's boxes have no velocity (nd != 9).
+
+        block=False returns a PendingResult, as infer_host's."""
         if n_feat + 1 != self.num_point_features:
             raise ValueError("ingested clouds have n_feat + 1 = %d features, the reader takes %d"
                              % (n_feat + 1, self.num_point_features))
@@ -332,9 +396,9 @@ class InferencePipeline:
             return packed if nusc is None else e.nusc.launch(packed)
         if nusc is None:
             return self._serve(graphed, key, make, step, self._packed_into(pinned_out), stage,
-                               fits=lambda e: e.ingest.radius == radius)
-        return nusc.annos(self._serve(graphed, ("sweeps_nusc",) + key, make, step, _NuscStep.fetch, stage,
-                                      fits=lambda e: e.ingest.radius == radius))
+                               fits=lambda e: e.ingest.radius == radius, block=block)
+        return self._serve(graphed, ("sweeps_nusc",) + key, make, step, self._rows_into, stage,
+                           fits=lambda e: e.ingest.radius == radius, finish=nusc.annos, block=block)
 
     # ---- raw KITTI scans: camera-frustum crop on the device ----------------------------------------------------------
     @staticmethod
@@ -418,7 +482,7 @@ class InferencePipeline:
         return [n for t in self.cfg.tasks for n in t["class_names"]]
 
     @torch.no_grad()
-    def infer_raw(self, clouds, calibs, pinned_out=None, graphed=False, kitti_results=False):
+    def infer_raw(self, clouds, calibs, pinned_out=None, graphed=False, kitti_results=False, block=True):
         """Raw KITTI scans -> host detections [B, D, nd+3], as infer_host: each scan is first cropped to its camera's
         view frustum (box_np_ops.remove_outside_points, bit-exact), on the device.
 
@@ -439,7 +503,9 @@ class InferencePipeline:
         name (self.class_names()).  d3b_kitti_results_dev runs right after predict, inside the same graph when
         graphed (keyed ("frustum_kitti", B, raw bucket, ndim), apart from the plain one); each scan's calibration table
         (kitti_calib_table, cached per calibration) goes H2D only when it differs from that graph's last replay, and
-        the kept rows, their counts and the f16-range flag come back in one D2H before one sync."""
+        the kept rows, their counts and the f16-range flag come back in one D2H before one sync.
+
+        block=False returns a PendingResult, as infer_host's; each unfinished frame has its own pinned result rows."""
         clouds, calibs = list(clouds), list(calibs)
         ndim, sizes = self.check_raw_clouds(clouds, calibs)
         planes = np.stack([self.frustum_planes(c) for c in calibs])
@@ -465,18 +531,12 @@ class InferencePipeline:
             packed = self.pack(self.forward_device(*e.crop.launch()))
             return packed if e.kitti is None else e.kitti.launch(packed)
 
-        def fetch(e, out):
-            if e.kitti is None:
-                return packed_into(e, out)
-            e.kitti.results_host.copy_(out[0], non_blocking=True)
-            e.kitti.counts_host.copy_(out[1], non_blocking=True)
-            return e.kitti
-        packed_into = self._packed_into(pinned_out)
         key = ("frustum_kitti" if kitti_results else "frustum", batch, bucket, ndim)
-        got = self._serve(graphed, key, make, step, fetch, stage)
-        if kitti_results:
-            return to_annos(got.results_host.numpy(), got.counts_host.numpy(), self.class_names())
-        return got
+        if not kitti_results:
+            return self._serve(graphed, key, make, step, self._packed_into(pinned_out), stage, block=block)
+        names = self.class_names()
+        return self._serve(graphed, key, make, step, self._rows_into, stage, block=block,
+                           finish=lambda got: to_annos(got[0].numpy(), got[1].numpy(), names))
 
     @staticmethod
     def unpack(packed_host):
@@ -491,7 +551,7 @@ class InferencePipeline:
 class _NuscStep:
     """infer_sweeps' and SweepStream.infer's nuScenes results post-step.  The constructor checks the arguments and
     builds the pose tables (ValueError before anything is enqueued); attach adds a NuscResults and its pose _Upload to a
-    new entry, stage uploads the poses when they changed, fetch enqueues the D2H of the rows, annos formats them."""
+    new entry, stage uploads the poses when they changed, annos formats the fetched (results, counts)."""
 
     def __init__(self, pipe, batch, poses, tokens):
         if poses is None or tokens is None:
@@ -518,13 +578,60 @@ class _NuscStep:
     def stage(self, entry):
         entry.pose_uploads += entry.poses.put(self.poses)
 
-    @staticmethod
-    def fetch(entry, _out):
-        return entry.nusc.fetch()
+    def annos(self, got):
+        return to_nusc_annos(got[0].numpy(), got[1].numpy(), self.class_names, self.tokens, self.table)
 
-    def annos(self, nusc):
-        return to_nusc_annos(nusc.results_host.numpy(), nusc.counts_host.numpy(), self.class_names, self.tokens,
-                             self.table)
+
+class PendingResult:
+    """One frame an InferencePipeline entry point submitted with block=False.  result() waits for it (completing the
+    pipeline's older unfinished frames first, in submission order) and returns exactly what the blocking call would
+    have: the packed host tensor, the KITTI anno dicts or the nusc_annos dict.  Results may be collected in any order
+    and more than once.  done() polls, without blocking, whether the frame has finished on the device (result() may
+    still re-run it on tf32x3 after an f16-range overflow).  rerun tells whether it was re-run."""
+
+    def __init__(self, pipe, run, finish, release):
+        self._pipe, self._run, self._finish, self._release = pipe, run, finish, release
+        self._bufs = {}                           # this frame's pinned host outputs by name, kept across a re-run
+        self._event = torch.cuda.Event()
+        self._entry = self._host = self._value = self._error = None
+        self._done = False
+        self.rerun = False
+
+    def _launch(self):
+        # the frame holds its entry until it completes: an evicted or dropped graph outlives its last replay
+        self._entry, self._host = self._run(self)
+        self._event.record()
+
+    def pinned(self, name, like):
+        """The frame's pinned host buffer `name`, shaped like the device tensor `like` (from the pipeline's pool)."""
+        buf = self._bufs.get(name)
+        if buf is None:
+            buf = self._bufs[name] = self._pipe._pinned_take(like.shape, like.dtype)
+        return buf
+
+    def _finish_now(self):
+        try:
+            self._value = self._host if self._finish is None else self._finish(self._host)
+        except Exception as err:                  # e.g. to_nusc_annos' NaN check: raised by this frame's result()
+            self._error = err
+        finally:
+            self._done = True
+            for buf in self._bufs.values():
+                self._pipe._pinned_give(buf)
+            if self._release is not None:
+                self._release()
+            self._bufs = {}
+            self._run = self._finish = self._release = self._entry = self._host = None
+
+    def done(self):
+        return self._done or self._event.query()
+
+    def result(self):
+        while not self._done:
+            self._pipe._complete_oldest()
+        if self._error is not None:
+            raise self._error
+        return self._value
 
 
 class _GraphEntry:
@@ -582,17 +689,26 @@ class SweepStream:
     the last bits.
 
     With graphed=True one CUDA graph keyed ("stream", B, K, slot_capacity, raw_stride, n_feat) in the pipeline's LRU
-    covers ingest, voxelize and forward.  Its raw capacity is B * K * slot_capacity, so frames of any size replay it;
-    the slot copies happen outside it.  A graph holds one stream's buffers: a second stream of the same shape on the same
-    pipeline replaces the entry (and recaptures) when it infers."""
+    covers ingest, voxelize and forward.  Its raw capacity is B * S * slot_capacity (S slots per stream), so frames of
+    any size replay it; the slot copies happen outside it.  A graph holds one stream's buffers: a second stream of the
+    same shape on the same pipeline replaces the entry (and recaptures) when it infers.
 
-    def __init__(self, pipe, batch, history=10, slot_capacity=40000, raw_stride=5, n_feat=4, radius=1.0):
+    infer(block=False) leaves frames in flight (InferencePipeline.max_in_flight).  An unfinished frame may still have to
+    be re-run from its slots (f16-range overflow), so it holds them until its result is collected, and push() refuses
+    (ValueError) to overwrite a held slot.  in_flight=k gives each stream S = K + k - 1 slots: a push then always finds
+    its slot free while at most k - 1 frames are unfinished, so frames can be pushed and submitted with k in flight.
+    The default, in_flight=1, keeps S = K and the key above; any other adds ("in_flight", k) to it."""
+
+    def __init__(self, pipe, batch, history=10, slot_capacity=40000, raw_stride=5, n_feat=4, radius=1.0, in_flight=1):
         if not 1 <= batch <= MAX_BATCH:
             raise ValueError("batch must be in [1, %d], got %d" % (MAX_BATCH, batch))
         if not 1 <= history <= MAX_SWEEPS:
             raise ValueError("history must be in [1, %d] sweeps (key frame included), got %d" % (MAX_SWEEPS, history))
-        if slot_capacity < 1 or batch * history * slot_capacity > 1 << 30:
-            raise ValueError("slot_capacity %d outside [1, 2^30 / (batch * history)]" % slot_capacity)
+        if not isinstance(in_flight, numbers.Integral) or in_flight < 1:
+            raise ValueError("in_flight must be an int >= 1, got %r" % (in_flight,))
+        slots = history + in_flight - 1
+        if slot_capacity < 1 or batch * slots * slot_capacity > 1 << 30:
+            raise ValueError("slot_capacity %d outside [1, 2^30 / (batch * (history + in_flight - 1))]" % slot_capacity)
         if n_feat < 3 or raw_stride < n_feat:
             raise ValueError("bad layout: n_feat %d, raw_stride %d" % (n_feat, raw_stride))
         if n_feat + 1 != pipe.num_point_features:
@@ -601,7 +717,9 @@ class SweepStream:
         self.pipe, self.batch, self.history, self.slot_capacity = pipe, batch, history, slot_capacity
         self.raw_stride, self.n_feat, self.radius = raw_stride, n_feat, radius
         self.key = ("stream", batch, history, slot_capacity, raw_stride, n_feat)
-        self.sweeps = SweepHistory(batch, history)
+        if in_flight != 1:
+            self.key += (("in_flight", in_flight),)
+        self.sweeps = SweepHistory(batch, history, slots)
         self.pending_h2d_bytes = 0                # pushed since the last infer()
         self.last_h2d_bytes = 0                   # of the last infer(): the pushes before it + its table
         self._ingest = None                       # device buffers, allocated on the first push
@@ -610,17 +728,19 @@ class SweepStream:
         """The gather BatchedIngest whose raw buffer holds the slots, and the slots' [B, K, slot_capacity, raw_stride]
         view of it (allocated on first use)."""
         if self._ingest is None:
-            B, K = self.batch, self.history
-            self._ingest = BatchedIngest(B, B * K * self.slot_capacity, B * K, self.raw_stride, self.n_feat, self.radius,
+            B, K, S = self.batch, self.history, self.sweeps.slots
+            self._ingest = BatchedIngest(B, B * S * self.slot_capacity, B * K, self.raw_stride, self.n_feat, self.radius,
                                          self.pipe.device, gather=True)
-            self._slots = self._ingest.raw.view(B, K, self.slot_capacity, self.raw_stride)
+            self._slots = self._ingest.raw.view(B, S, self.slot_capacity, self.raw_stride)
             self._table = _Upload(self._ingest.table)
             self._rows = [RowStager() for _ in range(B)]            # one staging buffer [slot_capacity] per stream
         return self._ingest, self._slots
 
     def check_push(self, b, raw, pose, timestamp):
-        """Host-side validation of push()'s arguments: raises ValueError.  Returns the number of raw points."""
+        """Host-side validation of push()'s arguments, and of the slot it would overwrite (SweepHistory.check_free):
+        raises ValueError.  Returns the number of raw points."""
         self.sweeps.check_stream(b)
+        self.sweeps.check_free(b)
         if torch.is_tensor(raw):
             ok = raw.dtype == torch.float32 and raw.device.type == "cpu"
         else:
@@ -640,8 +760,8 @@ class SweepStream:
     def push(self, b, raw, pose, timestamp):
         """Stream b's new sweep, which becomes its key frame: raw float32 [n, raw_stride] host array or tensor (pinned
         tensors are copied directly and must stay unchanged until the copy has run), pose the sensor-to-world 4x4
-        matrix, timestamp in seconds.  Enqueues one H2D copy into the stream's oldest slot; ValueError before anything
-        is enqueued when an argument is malformed."""
+        matrix, timestamp in seconds.  Enqueues one H2D copy into the stream's next slot; ValueError before anything
+        is enqueued when an argument is malformed or an unfinished frame still reads that slot."""
         rows = self.check_push(b, raw, pose, timestamp)
         _ing, slots = self._buffers()
         self._rows[b].put([raw], slots[b, self.sweeps.next_slot(b)])
@@ -660,19 +780,20 @@ class SweepStream:
         return [([slots[b, k, :n].cpu().numpy() for k, n in zip(ks, ns)], tms, lags)
                 for b, (ks, ns, tms, lags) in enumerate(frame)]
 
-    def _stage_table(self):
-        """Enqueues the H2D copy of the current frame's sweep table (every frame: it changes with each push)."""
-        frame = self.sweeps.frame()
+    def _frame_table(self, frame):
+        """The host image of `frame`'s sweep table (SweepHistory.frame()), which goes H2D every frame: it changes with
+        each push."""
         ing, _slots = self._buffers()
-        K, cap = self.history, self.slot_capacity
-        src = [(b * K + k) * cap for b, (ks, _ns, _tms, _lags) in enumerate(frame) for k in ks]
-        self._table.put(ing.host_table([(None, tms, lags) for _ks, _ns, tms, lags in frame],
-                                       [ns for _ks, ns, _tms, _lags in frame], sweep_src=src), always=True)
+        S, cap = self.sweeps.slots, self.slot_capacity
+        src = [(b * S + k) * cap for b, (ks, _ns, _tms, _lags) in enumerate(frame) for k in ks]
+        table = ing.host_table([(None, tms, lags) for _ks, _ns, tms, lags in frame],
+                               [ns for _ks, ns, _tms, _lags in frame], sweep_src=src)
         self.last_h2d_bytes = self.pending_h2d_bytes + ing.table.numel()
         self.pending_h2d_bytes = 0
+        return table
 
     @torch.no_grad()
-    def infer(self, pinned_out=None, graphed=False, nusc_results=False, poses=None, tokens=None):
+    def infer(self, pinned_out=None, graphed=False, nusc_results=False, poses=None, tokens=None, block=True):
         """Detections of the current frame, host [B, D, nd+3] as infer_sweeps returns them, and bit-identical to
         infer_sweeps(samples()).  The only H2D is the sweep table (the sweeps went with push).  graphed=True replays the
         stream's CUDA graph.  On an f16-range overflow the model switches to tf32x3 and the same frame is re-run, as in
@@ -680,16 +801,31 @@ class SweepStream:
 
         nusc_results=True (with poses and tokens, one per stream) returns the frame's nusc_annos as
         infer_sweeps(samples(), nusc_results=True) does, from the stream's graph keyed key + ("nusc",); the pose table
-        goes H2D only when it changed."""
+        goes H2D only when it changed.
+
+        block=False returns a PendingResult, as InferencePipeline.infer_host's; the frame holds its slots until then
+        (see the class)."""
         pipe = self.pipe
         nusc = _NuscStep(pipe, self.batch, poses, tokens) if nusc_results else None
-        self._stage_table()
+        frame = self.sweeps.frame()
+        table = self._frame_table(frame)
+
+        def stage(e):
+            self._table.put(table, always=True)
+            if nusc is not None:
+                nusc.stage(e)
 
         def step(e):
             packed = pipe.pack(pipe.forward_device(*self._ingest.launch()))
             return packed if nusc is None else e.nusc.launch(packed)
         if nusc is None:
-            return pipe._serve(graphed, self.key, lambda: _GraphEntry(stream=self), step, pipe._packed_into(pinned_out),
-                               fits=lambda e: e.stream is self)
-        return nusc.annos(pipe._serve(graphed, self.key + ("nusc",), lambda: nusc.attach(_GraphEntry(stream=self)),
-                                      step, _NuscStep.fetch, nusc.stage, fits=lambda e: e.stream is self))
+            key, make, fetch, finish = self.key, lambda: _GraphEntry(stream=self), pipe._packed_into(pinned_out), None
+        else:
+            key, make, fetch = self.key + ("nusc",), lambda: nusc.attach(_GraphEntry(stream=self)), pipe._rows_into
+            finish = nusc.annos
+
+        def hold():
+            held = self.sweeps.acquire(frame)
+            return lambda: self.sweeps.release(held)
+        return pipe._serve(graphed, key, make, step, fetch, stage, fits=lambda e: e.stream is self, finish=finish,
+                           block=block, hold=hold)

@@ -195,22 +195,51 @@ def stream_transforms(poses, timestamps):
 
 
 class SweepHistory:
-    """Host bookkeeping of B sweep histories of K slots each (apis.SweepStream keeps the sweeps themselves on the
-    device).  A push goes to slot (pushes since the last reset) mod K of its stream, so the slot it overwrites is the
-    stream's oldest once K sweeps are held; reset(b) forgets stream b's sweeps."""
+    """Host bookkeeping of B sweep histories of K sweeps each, kept in S >= K slots per stream (apis.SweepStream keeps
+    the sweeps themselves on the device).  A push goes to slot (pushes since the last reset) mod S of its stream, so
+    the slot it overwrites held the stream's (S - K + 1)-th oldest sweep once S sweeps were pushed; reset(b) forgets
+    stream b's sweeps.
 
-    def __init__(self, batch, history):
+    Frames that have not finished -- they may still have to be re-run from their slots -- hold their slots (acquire /
+    release); check_free refuses a push into a held slot.  With S = K + k - 1 a push finds its slot free while at most
+    k - 1 frames are unfinished, so with one more frame submitted after the push, k frames can be in flight."""
+
+    def __init__(self, batch, history, slots=None):
         self.batch, self.history = batch, history
+        self.slots = history if slots is None else int(slots)
+        if self.slots < history:
+            raise ValueError("%d slots cannot hold a history of %d sweeps" % (self.slots, history))
         self.count = [0] * batch                  # pushes since the last reset
         # per stream, oldest first: (slot, rows, pose f64 [4, 4], timestamp) of the sweeps still held
         self.held = [collections.deque(maxlen=history) for _ in range(batch)]
+        self.readers = [[0] * self.slots for _ in range(batch)]      # unfinished frames reading each slot
 
     def check_stream(self, b):
         if not isinstance(b, numbers.Integral) or not 0 <= b < self.batch:
             raise ValueError("stream index %r outside [0, %d)" % (b, self.batch))
 
     def next_slot(self, b):
-        return self.count[b] % self.history
+        return self.count[b] % self.slots
+
+    def check_free(self, b):
+        """ValueError when stream b's next push would overwrite a slot an unfinished frame reads."""
+        slot = self.next_slot(b)
+        if self.readers[b][slot]:
+            raise ValueError("stream %d: the next push would overwrite slot %d, which %d unfinished frame(s) read; "
+                             "collect the oldest frame's result first (or give the stream more in_flight)"
+                             % (b, slot, self.readers[b][slot]))
+
+    def acquire(self, frame):
+        """Marks the slots of `frame` (frame()'s value) as read by one more unfinished frame.  Returns the
+        (stream, slot) pairs to pass to release once that frame has finished."""
+        held = [(b, k) for b, (ks, _ns, _tms, _lags) in enumerate(frame) for k in ks]
+        for b, k in held:
+            self.readers[b][k] += 1
+        return held
+
+    def release(self, held):
+        for b, k in held:
+            self.readers[b][k] -= 1
 
     def record(self, b, rows, pose, timestamp):
         """Books stream b's new sweep into next_slot(b), which it returns."""

@@ -51,7 +51,8 @@ def to_annos(results, counts, class_names):
     """Host results [B, D, 14] f64 and counts [B] -> one anno dict per frame with the reference's keys and dtypes (names
     str, truncated f64, occluded int64, alpha f64, bbox f64 [n, 4], dimensions / location f64 [n, 3], rotation_y f64,
     score f32), or empty_result_anno() for a frame with none.  The arrays are copies."""
-    class_names = list(class_names)
+    names = np.empty(len(class_names), object)
+    names[:] = list(class_names)
     annos = []
     for rows, n in zip(np.asarray(results), np.asarray(counts)):
         n = int(n)
@@ -59,7 +60,8 @@ def to_annos(results, counts, class_names):
             annos.append(empty_result_anno())
             continue
         r = rows[:n]
-        annos.append(dict(name=np.array([class_names[int(k)] for k in r[:, 13]]), truncated=np.zeros(n),
+        # np.array of the names as a list: its dtype is as wide as the longest name kept, not the longest class
+        annos.append(dict(name=np.array(names[r[:, 13].astype(np.int64)].tolist()), truncated=np.zeros(n),
                           occluded=np.zeros(n, np.int64), alpha=r[:, 4].copy(), bbox=r[:, 0:4].copy(),
                           dimensions=r[:, 5:8].copy(), location=r[:, 8:11].copy(), rotation_y=r[:, 11].copy(),
                           score=r[:, 12].astype(np.float32)))

@@ -119,19 +119,23 @@ def to_nusc_annos(results, counts, class_names, tokens, table=None):
     ValueError for a class name without an attribute, and for a row whose translation or size is NaN (the devkit's
     Box asserts on a NaN centre or size)."""
     table = attribute_table(class_names) if table is None else table
-    class_names = list(class_names)
+    # object arrays of the caller's own str objects: a fancy index then .tolist() hands back those objects
+    names = np.empty(len(class_names), object)
+    names[:] = list(class_names)
+    attrs = np.empty((len(table), 2), object)
+    attrs[:] = [tuple(t) for t in table]
     out = {}
     for token, rows, n in zip(tokens, np.asarray(results), np.asarray(counts)):
         r = rows[:int(n)]
         if np.isnan(r[:, 0:6]).any():
             raise ValueError("sample %r: a detection with a NaN centre or size" % (token,))
-        annos = []
-        for row in r.tolist():
-            label = int(row[13])
-            annos.append({"sample_token": token, "translation": row[0:3], "size": row[3:6], "rotation": row[6:10],
-                          "velocity": row[10:12], "detection_name": class_names[label], "detection_score": row[12],
-                          "attribute_name": table[label][row[14] > 0.5]})
-        out[token] = annos
+        labels = r[:, 13].astype(np.int64)                              # int() of each label: truncation
+        moving = (r[:, 14] > 0.5).astype(np.intp)
+        out[token] = [{"sample_token": token, "translation": t, "size": s, "rotation": q, "velocity": v,
+                       "detection_name": nm, "detection_score": sc, "attribute_name": at}
+                      for t, s, q, v, nm, sc, at in zip(r[:, 0:3].tolist(), r[:, 3:6].tolist(), r[:, 6:10].tolist(),
+                                                        r[:, 10:12].tolist(), names[labels].tolist(), r[:, 12].tolist(),
+                                                        attrs[labels, moving].tolist())]
     return {"results": out, "meta": dict(META)}
 
 
