@@ -7,6 +7,9 @@
 //   SubMConv3d : outputs == inputs (same rows, same order), padding = k/2
 //   SparseConv3d: outputs = every in-bounds o reachable from an active p,
 //                 numbered by ascending linear index ((b*D+z)*H+y)*W+x.
+// Row rule, the same in every kernel here and in the scatters: a row whose batch index or coordinate lies outside its
+// grid is ignored (it is no neighbour, marks no output and gets -1 for every offset), and among rows that share a
+// cell the lowest row index is the one every lookup returns.
 //
 // The map is stored output-stationary (nbr[k][o] = input row or -1) so the
 // convolution kernel owns its output rows: no scatter-add, no atomics,
@@ -51,6 +54,11 @@ __device__ __forceinline__ unsigned long long lin_index(const SiteIndexDev& s, i
   return (((unsigned long long)b * s.D + z) * s.H + y) * s.W + x;
 }
 
+__device__ __forceinline__ bool in_grid(const SiteIndexDev& s, int4 c) {
+  return (unsigned)c.x < (unsigned)s.B && (unsigned)c.y < (unsigned)s.D && (unsigned)c.z < (unsigned)s.H &&
+         (unsigned)c.w < (unsigned)s.W;
+}
+
 __device__ __forceinline__ int site_lookup(const SiteIndexDev& s, int b, int z, int y, int x) {
   if ((unsigned)z >= (unsigned)s.D || (unsigned)y >= (unsigned)s.H || (unsigned)x >= (unsigned)s.W)
     return -1;
@@ -78,15 +86,15 @@ struct KernelGeom {
 };
 
 // ---- level-0 hash build --------------------------------------------------------
+// vals must hold a value above every row index on entry (0x7f memset): duplicates of a cell keep the lowest row, so
+// the map does not depend on which thread wins the key.
 __global__ void __launch_bounds__(256)
 rb_hash_insert(const int* __restrict__ coors, const int* __restrict__ n_rows, int row_cap,
                SiteIndexDev s, unsigned long long* keys, int* vals) {
   const int n = min(*n_rows, row_cap);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const int4 c = *reinterpret_cast<const int4*>(coors + (size_t)i * 4);
-    if ((unsigned)c.x >= (unsigned)s.B || (unsigned)c.y >= (unsigned)s.D ||
-        (unsigned)c.z >= (unsigned)s.H || (unsigned)c.w >= (unsigned)s.W)
-      continue;  // out-of-grid rows are never found by any lookup
+    if (!in_grid(s, c)) continue;  // out-of-grid rows are never found by any lookup
     const unsigned long long lin = lin_index(s, c.x, c.y, c.z, c.w);
     unsigned int slot = (unsigned int)mix64(lin) & s.hmask;
     while (true) {
@@ -94,7 +102,7 @@ rb_hash_insert(const int* __restrict__ coors, const int* __restrict__ n_rows, in
       if (prev == kEmptyKey || prev == lin) break;
       slot = (slot + 1) & s.hmask;
     }
-    vals[slot] = i;
+    atomicMin(&vals[slot], i);
   }
 }
 
@@ -103,7 +111,7 @@ rb_hash_insert(const int* __restrict__ coors, const int* __restrict__ n_rows, in
 // both the coordinate reads and the nbr writes are coalesced.
 __global__ void __launch_bounds__(256)
 rb_neighbours(const int* __restrict__ out_coors, const int* __restrict__ n_out, int out_cap,
-              SiteIndexDev in_index, KernelGeom g, int* __restrict__ nbr,
+              SiteIndexDev out_grid, SiteIndexDev in_index, KernelGeom g, int* __restrict__ nbr,
               unsigned int* __restrict__ tile_mask) {
   const int n = min(*n_out, out_cap);
   const long long total = (long long)n * g.kvol;
@@ -118,7 +126,7 @@ rb_neighbours(const int* __restrict__ out_coors, const int* __restrict__ n_out, 
     const int z = c.y * g.s[0] - g.p[0] + kz;
     const int y = c.z * g.s[1] - g.p[1] + ky;
     const int x = c.w * g.s[2] - g.p[2] + kx;
-    const int r = site_lookup(in_index, c.x, z, y, x);
+    const int r = in_grid(out_grid, c) ? site_lookup(in_index, c.x, z, y, x) : -1;
     nbr[(size_t)k * out_cap + o] = r;
     if (r >= 0) {
       // one atomic per (tile, k) group present in this warp
@@ -132,7 +140,7 @@ rb_neighbours(const int* __restrict__ out_coors, const int* __restrict__ n_out, 
 // ---- strided conv: mark reachable output sites --------------------------------------
 __global__ void __launch_bounds__(256)
 rb_mark_outputs(const int* __restrict__ in_coors, const int* __restrict__ n_in, int in_cap,
-                SiteIndexDev out, KernelGeom g, unsigned int* bitmap) {
+                SiteIndexDev in_dims, SiteIndexDev out, KernelGeom g, unsigned int* bitmap) {
   const int n = min(*n_in, in_cap);
   const long long total = (long long)n * g.kvol;
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total;
@@ -140,7 +148,7 @@ rb_mark_outputs(const int* __restrict__ in_coors, const int* __restrict__ n_in, 
     const int i = (int)(e / g.kvol);
     const int k = (int)(e - (long long)i * g.kvol);
     const int4 c = *reinterpret_cast<const int4*>(in_coors + (size_t)i * 4);
-    if ((unsigned)c.x >= (unsigned)out.B) continue;
+    if (!in_grid(in_dims, c)) continue;
     const int kx = k % g.k[2];
     const int ky = (k / g.k[2]) % g.k[1];
     const int kz = k / (g.k[2] * g.k[1]);
@@ -309,6 +317,7 @@ extern "C" int d3b_index_build_hash(const int32_t* coors, const int32_t* n_rows,
               "d3b_index_build_hash: hash_cap %d must be a power of two >= 2*row_cap (%d)",
               index->hash_cap, row_cap);
   D3B_CUDA(cudaMemsetAsync(index->hash_keys, 0xff, (size_t)index->hash_cap * 8, stream));
+  D3B_CUDA(cudaMemsetAsync(index->hash_vals, 0x7f, (size_t)index->hash_cap * 4, stream));  // > any row (atomicMin)
   SiteIndexDev s = to_dev(index, row_cap);
   rb_hash_insert<<<grid_for(row_cap, 256), 256, 0, stream>>>(
       coors, n_rows, row_cap, s, (unsigned long long*)index->hash_keys, index->hash_vals);
@@ -329,8 +338,9 @@ extern "C" int d3b_rulebook_subm(const int32_t* coors, const int32_t* n_rows, in
     g.p[j] = ksize[j] / 2;
   }
   D3B_CUDA(cudaMemsetAsync(tile_mask, 0, (size_t)div_up(row_cap, 128) * 4, stream));
-  rb_neighbours<<<grid_for((long long)row_cap * g.kvol, 256), 256, 0, stream>>>(
-      coors, n_rows, row_cap, to_dev(index, row_cap), g, nbr, tile_mask);
+  const SiteIndexDev s = to_dev(index, row_cap);
+  rb_neighbours<<<grid_for((long long)row_cap * g.kvol, 256), 256, 0, stream>>>(coors, n_rows, row_cap, s, s, g, nbr,
+                                                                               tile_mask);
   D3B_LAUNCH_CHECK();
   return D3B_OK;
 }
@@ -350,6 +360,9 @@ extern "C" int d3b_rulebook_conv(const int32_t* in_coors, const int32_t* n_in, i
   D3B_REQUIRE(check_geom(ksize, &g) == 0, "d3b_rulebook_conv: kernel volume must be in [1,32]");
   for (int j = 0; j < 3; ++j) {
     D3B_REQUIRE(stride[j] >= 1 && padding[j] >= 0, "d3b_rulebook_conv: bad stride/padding");
+    D3B_REQUIRE(in_index->spatial[j] + 2 * padding[j] >= ksize[j],
+                "d3b_rulebook_conv: kernel %d wider than the padded input %d + 2*%d along axis %d", ksize[j],
+                in_index->spatial[j], padding[j], j);
     g.s[j] = stride[j];
     g.p[j] = padding[j];
     const int expect = (in_index->spatial[j] + 2 * padding[j] - (ksize[j] - 1) - 1) / stride[j] + 1;
@@ -374,7 +387,7 @@ extern "C" int d3b_rulebook_conv(const int32_t* in_coors, const int32_t* n_in, i
   D3B_CUDA(cudaMemsetAsync(out_index->bitmap, 0, (size_t)n_words * 4, stream));
   D3B_CUDA(cudaMemsetAsync(tile_mask, 0, (size_t)div_up(out_cap, 128) * 4, stream));
   rb_mark_outputs<<<grid_for((long long)in_cap * g.kvol, 256), 256, 0, stream>>>(
-      in_coors, n_in, in_cap, out, g, out_index->bitmap);
+      in_coors, n_in, in_cap, to_dev(in_index, in_cap), out, g, out_index->bitmap);
   D3B_LAUNCH_CHECK();
   D3B_CUDA(cudaMemsetAsync(block_sums, 0xff, (size_t)n_blocks * 4, stream));       // -1 = "not published yet"
   rb_scan_fused<<<n_blocks, kScanThreads, 0, stream>>>(out_index->bitmap, n_words, block_sums, out_cap, n_out,
@@ -384,7 +397,7 @@ extern "C" int d3b_rulebook_conv(const int32_t* in_coors, const int32_t* n_in, i
                                                            out_cap, out_coors);
   D3B_LAUNCH_CHECK();
   rb_neighbours<<<grid_for((long long)out_cap * g.kvol, 256), 256, 0, stream>>>(
-      out_coors, n_out, out_cap, to_dev(in_index, in_cap), g, nbr, tile_mask);
+      out_coors, n_out, out_cap, out, to_dev(in_index, in_cap), g, nbr, tile_mask);
   D3B_LAUNCH_CHECK();
   return D3B_OK;
 }

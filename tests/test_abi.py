@@ -145,3 +145,19 @@ def test_pillar_reader_rejects_unbuilt_shapes_without_gpu():
         assert call(4, 2600, 5, 64) == 1 and b"shared memory" in L.d3b_last_error()
     assert lists(65, 20, 4, 64) == 1 and b"batch 65" in L.d3b_last_error()
     assert lists(0, 20, 4, 64) == 1 and b"batch 0" in L.d3b_last_error()
+
+
+def test_rulebook_conv_rejects_a_kernel_wider_than_the_padded_input():
+    """D = 1, k = 2, padding 0: there is no output cell along z (floor((1 - 2) / 2) + 1 = 0); C's truncating division
+    would make it 1, an output whose window leaves the grid.  Rejected before any CUDA call."""
+    host = (ctypes.c_int32 * 16)()
+    buf = ctypes.addressof(host)
+    i3 = lambda *v: (ctypes.c_int32 * 3)(*v)
+    in_idx, out_idx = _lib.SiteIndex(), _lib.SiteIndex()
+    in_idx.spatial, in_idx.batch = i3(1, 8, 8), 1
+    out_idx.spatial, out_idx.batch = i3(1, 4, 4), 1
+    out_idx.bitmap, out_idx.word_prefix, out_idx.n_words = buf, buf, 1
+    st = _lib.lib().d3b_rulebook_conv(buf, buf, 1, ctypes.byref(in_idx), i3(2, 2, 2), i3(2, 2, 2), i3(0, 0, 0),
+                                      ctypes.byref(out_idx), buf, buf, 1, buf, buf, buf, 64, None)
+    assert st == 1
+    assert b"wider than the padded input" in _lib.lib().d3b_last_error()

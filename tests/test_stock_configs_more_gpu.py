@@ -236,8 +236,11 @@ def test_forward_launches_no_vendor_kernel(deployed, name):
     cfg, pipe, _cpu, _sd, run = deployed(name)
     pipe.forward_device(run["pts"], run["offsets"])
     torch.cuda.synchronize()
+    # two forwards per trace: a trace can lack the device records of its first operations (see
+    # test_frustum_gpu.test_graphed_forward_runs_no_vendor_kernel), and spconv_first16 runs right after the voxelizer
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        pipe.forward_device(run["pts"], run["offsets"])
+        for _ in range(2):
+            pipe.forward_device(run["pts"], run["offsets"])
         torch.cuda.synchronize()
     names = {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
     ours = {n for n in names if "d3b" in n}
