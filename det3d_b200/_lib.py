@@ -117,14 +117,9 @@ SIGNATURES = {
     "d3b_set_bev_variant": (None, [C.c_int]),
     "d3b_get_bev_variant": (C.c_int, []),
     "d3b_voxelize_workspace_bytes": (_sz, [C.POINTER(VoxelCfg), _i32, _i32]),
-    "d3b_voxelize": (C.c_int, [C.POINTER(VoxelCfg), _vp, C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "d3b_voxelize_dev": (C.c_int, [C.POINTER(VoxelCfg), _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "d3b_ingest_workspace_bytes": (_sz, [_i32]),
-    "d3b_ingest_sweeps": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _vp, _i32, _vp, _vp, _sz, _vp]),
     "d3b_ingest_dev_workspace_bytes": (_sz, [_i32, _i32]),
-    "d3b_ingest_sweeps_dev": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "d3b_ingest_gather_workspace_bytes": (_sz, [_i32, _i32]),
-    "d3b_ingest_sweeps_gather": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "d3b_ingest_sweeps_dev": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _sz, _vp]),
     "d3b_frustum_crop_workspace_bytes": (_sz, [_i32, _i32]),
     "d3b_frustum_crop_dev": (C.c_int, [_vp, _i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
     "d3b_kitti_results_dev": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp]),

@@ -20,14 +20,15 @@ import torch
 from det3d_b200 import _lib
 from det3d_b200.core.anchor.anchor_generator import anchors_for_tasks
 from det3d_b200.core.bbox.box_np_ops import camera_frustum_planes
-from det3d_b200.datasets.pipelines.loading import (MAX_BATCH, MAX_SWEEPS, BatchedIngest, RowStager, SweepHistory,
-                                                    check_sweep_samples, sweep_table_capacity)
+from det3d_b200.datasets.pipelines.loading import (MAX_BATCH, MAX_SWEEPS, BatchedIngest, SweepHistory, check_sweep_samples,
+                                                    sweep_table_capacity)
 from det3d_b200.models import build_detector
 from det3d_b200.ops.point_cloud.frustum import MAX_NDIM, MIN_NDIM, FrustumCrop
 from det3d_b200.ops.point_cloud.kitti_results import KittiResults, calib_table, check_calibs, to_annos
 from det3d_b200.ops.point_cloud.nusc_results import (ND as NUSC_ND, NuscResults, attribute_table, check_tokens,
                                                      pose_table, to_nusc_annos)
 from det3d_b200.ops.point_cloud.voxelize import Voxelizer
+from det3d_b200.utils.staging import RowStager, Upload
 
 
 class InferencePipeline:
@@ -255,7 +256,7 @@ class InferencePipeline:
     def _points_entry(self, batch, bucket, ndim):
         """forward_graphed's entry (batch, bucket, ndim): static points [bucket, ndim] and device offsets [batch + 1]."""
         return _GraphEntry(points=torch.zeros((bucket, ndim), dtype=torch.float32, device=self.device), rows=RowStager(),
-                           offsets=_Upload(torch.zeros(batch + 1, dtype=torch.int32, device=self.device)))
+                           offsets=Upload(torch.zeros(batch + 1, dtype=torch.int32, device=self.device)))
 
     def _graph_entry(self, batch, n_points, ndim):
         """The graph-cache entry of (batch, bucket_of(n_points), ndim); a new entry has buffers but no graph yet."""
@@ -382,7 +383,7 @@ class InferencePipeline:
         def make():
             # eager too, the voxelizer's capacity is the bucket: it keeps its device-offset buffers per capacity
             ingest = BatchedIngest(*key, radius, self.device)
-            entry = _GraphEntry(ingest=ingest, table=_Upload(ingest.table), rows=RowStager())
+            entry = _GraphEntry(ingest=ingest, table=Upload(ingest.table), rows=RowStager())
             return entry if nusc is None else nusc.attach(entry)
 
         def stage(e):
@@ -516,8 +517,8 @@ class InferencePipeline:
         def make():
             crop = FrustumCrop(batch, bucket, ndim, self.device)
             kitti = KittiResults(batch, self.device) if kitti_results else None
-            return _GraphEntry(crop=crop, offsets=_Upload(crop.offsets), planes=_Upload(crop.planes), rows=RowStager(),
-                               kitti=kitti, calib=None if kitti is None else _Upload(kitti.calib),
+            return _GraphEntry(crop=crop, offsets=Upload(crop.offsets), planes=Upload(crop.planes), rows=RowStager(),
+                               kitti=kitti, calib=None if kitti is None else Upload(kitti.calib),
                                planes_uploads=0, calib_uploads=0)          # H2D copies of each table so far
 
         def stage(e):
@@ -550,7 +551,7 @@ class InferencePipeline:
 
 class _NuscStep:
     """infer_sweeps' and SweepStream.infer's nuScenes results post-step.  The constructor checks the arguments and
-    builds the pose tables (ValueError before anything is enqueued); attach adds a NuscResults and its pose _Upload to a
+    builds the pose tables (ValueError before anything is enqueued); attach adds a NuscResults and its pose Upload to a
     new entry, stage uploads the poses when they changed, annos formats the fetched (results, counts)."""
 
     def __init__(self, pipe, batch, poses, tokens):
@@ -571,7 +572,7 @@ class _NuscStep:
 
     def attach(self, entry):
         entry.nusc = NuscResults(self.batch, self.device)
-        entry.poses = _Upload(entry.nusc.poses)
+        entry.poses = Upload(entry.nusc.poses)
         entry.pose_uploads = 0                        # H2D copies of the pose table so far
         return entry
 
@@ -636,38 +637,12 @@ class PendingResult:
 
 class _GraphEntry:
     """One entry point's state: the static buffers it attaches (points, a BatchedIngest, a FrustumCrop, a KittiResults,
-    their _Uploads and RowStager) and, once captured, the graph and its output.  A graphed entry lives in the graph
+    their Uploads and RowStager) and, once captured, the graph and its output.  A graphed entry lives in the graph
     cache; an eager one serves one call."""
 
     def __init__(self, **buffers):
         self.graph = self.out = None
         self.__dict__.update(buffers)
-
-
-class _Upload:
-    """A small device table `dev` that goes H2D only when its bytes change, through a pinned staging copy."""
-
-    def __init__(self, dev):
-        self.dev = dev
-        self.staging = torch.empty(dev.shape, dtype=dev.dtype, pin_memory=True)
-        self.copied = torch.cuda.Event()
-        self.last = None
-
-    def put(self, value, always=False):
-        """Enqueues the H2D copy of the host `value` (dev's shape, converted to its dtype) unless its bytes equal the
-        last put's; always=True copies in any case.  Returns whether it copied."""
-        host = self.staging.numpy()
-        value = np.asarray(value, host.dtype)
-        raw = value.tobytes()
-        if raw == self.last and not always:
-            return False
-        self.copied.synchronize()                 # the staging buffer may still feed the previous copy
-        host[...] = value
-        with torch.cuda.device(self.dev.device):
-            self.dev.copy_(self.staging, non_blocking=True)
-            self.copied.record()
-        self.last = raw
-        return True
 
 
 class SweepStream:
@@ -679,7 +654,7 @@ class SweepStream:
     In a frame the newest push of each stream is its key frame (neither filtered nor transformed) and its earlier sweeps
     follow newest first, each under inv(P_key) @ P_s (float64, on the host) with lag t_key - t_s rounded to float32 and
     the `radius` remove_close filter, exactly as infer_sweeps treats a sample.  infer() sends only the sweep table (a few
-    KB: offsets, slot starts, transforms, lags, flags) and runs d3b_ingest_sweeps_gather over the slots; the detections
+    KB: offsets, slot starts, transforms, lags, flags) and runs d3b_ingest_sweeps_dev over the slots; the detections
     are bit-identical to infer_sweeps(samples()).  A stream with fewer than K pushes uses the sweeps it has; reset(b)
     empties a stream (e.g. at a scene change).
 
@@ -732,7 +707,7 @@ class SweepStream:
             self._ingest = BatchedIngest(B, B * S * self.slot_capacity, B * K, self.raw_stride, self.n_feat, self.radius,
                                          self.pipe.device, gather=True)
             self._slots = self._ingest.raw.view(B, S, self.slot_capacity, self.raw_stride)
-            self._table = _Upload(self._ingest.table)
+            self._table = Upload(self._ingest.table)
             self._rows = [RowStager() for _ in range(B)]            # one staging buffer [slot_capacity] per stream
         return self._ingest, self._slots
 

@@ -35,7 +35,7 @@ void count_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memo
 }  // namespace d3b
 
 extern "C" const char* d3b_last_error(void) { return d3b::g_error; }
-extern "C" int d3b_abi_version(void) { return 4; }
+extern "C" int d3b_abi_version(void) { return 5; }
 extern "C" void d3b_set_pdl(int on) { d3b::g_pdl.store(on ? 1 : 0, std::memory_order_relaxed); }
 extern "C" void d3b_set_bev_variant(int v) { d3b::g_bev_variant.store(v == 0 ? 0 : 2, std::memory_order_relaxed); }
 extern "C" int d3b_get_bev_variant(void) { return d3b::bev_variant(); }

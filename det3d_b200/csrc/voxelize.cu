@@ -27,13 +27,12 @@
 // HBM traffic per cloud = N*ndim*4 (points, read twice: A and D, the second
 // time from L2) + M*(max_points*ndim*4 + 16 + 4 + ndim*4) written once.
 //
-// Cloud offsets: d3b_voxelize takes them on the host (in the by-value params),
-// d3b_voxelize_dev reads them from device memory, so one captured CUDA graph
-// serves clouds of any size up to a point capacity.  Either way every CTA
-// that needs them first copies them, and their 1024-point chunk prefix, into
-// shared memory (load_offsets).  The device path sizes its grids, the hash
-// and the workspace from the capacity; voxel ids are first-point ranks, not
-// hash slots, so its outputs are bit-identical to the host path's.
+// Cloud offsets: d3b_voxelize_dev reads them from device memory, so one
+// captured CUDA graph serves clouds of any size up to a point capacity.  Every
+// CTA that needs them first copies them, clamped, and their 1024-point chunk
+// prefix into shared memory (load_offsets).  Grids, hash and workspace are
+// sized from the capacity; voxel ids are first-point ranks, not hash slots, so
+// the outputs do not depend on the capacity.
 #include "common.cuh"
 
 namespace d3b {
@@ -47,10 +46,8 @@ struct VoxParams {
   float lo[3];
   int grid[3];
   int ndim, max_points, max_voxels, batch;
-  int off[kMaxBatch + 1];         // host offsets (d3b_voxelize)
-  int chunk_off[kMaxBatch + 1];   // rank chunks (1024 points) of the clouds, prefix
-  const int* off_dev;             // device offsets (d3b_voxelize_dev), else nullptr
-  int point_cap;                  // d3b_voxelize_dev: rows of `points`
+  const int* off_dev;             // device cloud offsets [batch + 1]
+  int point_cap;                  // rows of `points`
 };
 
 // Per-CTA copy of the cloud offsets and of their chunk prefix.
@@ -59,48 +56,44 @@ struct VoxOffsets {
   int chunk_off[kMaxBatch + 1];
 };
 
-// Fills `s` from the params (host offsets) or from p.off_dev.  Device offsets are clamped into
+// Fills `s` from p.off_dev, clamped into
 // 0 = off[0] <= ... <= off[batch] <= point_cap as off[b] = min(max(0, raw[1..b]), point_cap) -- the same values in every
 // CTA, before any point index is formed.  Returns (to every thread, after the barrier) whether the clamp changed anything.
 __device__ __forceinline__ bool load_offsets(const VoxParams& p, VoxOffsets& s) {
   __shared__ int s_bad;
   if (threadIdx.x < 32) {
     const int lane = threadIdx.x;
-    if (p.off_dev == nullptr) {
-      for (int b = lane; b <= p.batch; b += 32) { s.off[b] = p.off[b]; s.chunk_off[b] = p.chunk_off[b]; }
-      if (lane == 0) s_bad = 0;
-    } else {
-      int run_max = 0, run_off = 0, run_chunks = 0;
-      bool bad = false;
-      for (int base = 0; base <= p.batch; base += 32) {
-        const int b = base + lane;
-        const int raw = b <= p.batch ? __ldg(p.off_dev + b) : 0;
-        int m = b == 0 ? 0 : raw;                           // rows past `batch` repeat the last offset: 0 chunks
+    int run_max = 0, run_off = 0, run_chunks = 0;
+    bool bad = false;
+#pragma unroll 1                                            // unrolled, it raises every kernel's register count
+    for (int base = 0; base <= p.batch; base += 32) {
+      const int b = base + lane;
+      const int raw = b <= p.batch ? __ldg(p.off_dev + b) : 0;
+      int m = b == 0 ? 0 : raw;                             // rows past `batch` repeat the last offset: 0 chunks
 #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {                  // inclusive prefix max
-          const int t = __shfl_up_sync(0xffffffffu, m, d);
-          if (lane >= d) m = max(m, t);
-        }
-        m = max(m, run_max);
-        const int c = min(m, p.point_cap);
-        bad |= b <= p.batch && c != raw;
-        int prev = __shfl_up_sync(0xffffffffu, c, 1);
-        if (lane == 0) prev = run_off;
-        int n = b == 0 ? 0 : (c - prev + kRankChunk - 1) / kRankChunk;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {                  // inclusive prefix sum of the chunk counts
-          const int t = __shfl_up_sync(0xffffffffu, n, d);
-          if (lane >= d) n += t;
-        }
-        n += run_chunks;
-        if (b <= p.batch) { s.off[b] = c; s.chunk_off[b] = n; }
-        run_max = __shfl_sync(0xffffffffu, m, 31);
-        run_off = __shfl_sync(0xffffffffu, c, 31);
-        run_chunks = __shfl_sync(0xffffffffu, n, 31);
+      for (int d = 1; d < 32; d <<= 1) {                    // inclusive prefix max
+        const int t = __shfl_up_sync(0xffffffffu, m, d);
+        if (lane >= d) m = max(m, t);
       }
-      bad = __any_sync(0xffffffffu, bad);
-      if (lane == 0) s_bad = bad;
+      m = max(m, run_max);
+      const int c = min(m, p.point_cap);
+      bad |= b <= p.batch && c != raw;
+      int prev = __shfl_up_sync(0xffffffffu, c, 1);
+      if (lane == 0) prev = run_off;
+      int n = b == 0 ? 0 : (c - prev + kRankChunk - 1) / kRankChunk;
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {                    // inclusive prefix sum of the chunk counts
+        const int t = __shfl_up_sync(0xffffffffu, n, d);
+        if (lane >= d) n += t;
+      }
+      n += run_chunks;
+      if (b <= p.batch) { s.off[b] = c; s.chunk_off[b] = n; }
+      run_max = __shfl_sync(0xffffffffu, m, 31);
+      run_off = __shfl_sync(0xffffffffu, c, 31);
+      run_chunks = __shfl_sync(0xffffffffu, n, 31);
     }
+    bad = __any_sync(0xffffffffu, bad);
+    if (lane == 0) s_bad = bad;
   }
   __syncthreads();
   return s_bad != 0;
@@ -178,7 +171,7 @@ vox_chunk_count(const VoxParams p, const int* __restrict__ first, const int* __r
   __shared__ VoxOffsets s;
   load_offsets(p, s);
   const int g = blockIdx.x;
-  if (g >= s.chunk_off[p.batch]) return;   // d3b_voxelize_dev: grid sized for the capacity
+  if (g >= s.chunk_off[p.batch]) return;   // the grid is sized for the capacity
   const int b = chunk_cloud(p, s, g);
   const int i0 = s.off[b] + (g - s.chunk_off[b]) * kRankChunk + threadIdx.x * 4;
   int slot[4];
@@ -247,7 +240,7 @@ vox_assign(const VoxParams p, const int* __restrict__ first, const int* __restri
   __shared__ VoxOffsets s;
   load_offsets(p, s);
   const int g = blockIdx.x;
-  if (g >= s.chunk_off[p.batch]) return;   // d3b_voxelize_dev: grid sized for the capacity
+  if (g >= s.chunk_off[p.batch]) return;   // the grid is sized for the capacity
   const int b = chunk_cloud(p, s, g);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int i0 = s.off[b] + (g - s.chunk_off[b]) * kRankChunk + threadIdx.x * 4;
@@ -412,31 +405,12 @@ extern "C" const int32_t* d3b_voxelize_point_lists(const d3b_voxel_cfg* cfg, int
   return carve(cfg, n_points_total, batch, (char*)workspace).lists;
 }
 
-// The checks and launches both entry points share.  `n_rows` sizes the grid-stride kernels and `n_chunks` the rank-chunk
-// grids: the exact counts for host offsets, bounds derived from the capacity for device offsets (the kernels stop at the
-// live counts they read from the offsets).
-static int check_cfg(const d3b_voxel_cfg* cfg, int32_t batch, const char* fn) {
-  D3B_REQUIRE(batch >= 1 && batch <= kMaxBatch, "%s: batch %d outside [1,%d]", fn, batch, kMaxBatch);
-  D3B_REQUIRE(cfg->ndim >= 3 && cfg->max_points >= 1 && cfg->max_voxels >= 1,
-              "%s: bad cfg (ndim %d, max_points %d, max_voxels %d)", fn, cfg->ndim, cfg->max_points, cfg->max_voxels);
-  for (int j = 0; j < 3; ++j)
-    D3B_REQUIRE(cfg->grid[j] >= 1 && cfg->voxel_size[j] > 0.0f, "%s: bad grid/voxel_size", fn);
-  D3B_REQUIRE((double)cfg->grid[0] * cfg->grid[1] * cfg->grid[2] * batch < 9.0e18, "%s: grid too large", fn);
-  return D3B_OK;
-}
-
-static VoxParams params_of(const d3b_voxel_cfg* cfg, int32_t batch) {
-  VoxParams p;
-  for (int j = 0; j < 3; ++j) { p.vs[j] = cfg->voxel_size[j]; p.lo[j] = cfg->range_min[j]; p.grid[j] = cfg->grid[j]; }
-  p.ndim = cfg->ndim; p.max_points = cfg->max_points; p.max_voxels = cfg->max_voxels; p.batch = batch;
-  p.off_dev = nullptr;
-  p.point_cap = 0;
-  return p;
-}
-
-static int launch_voxelize(const VoxParams& p, const d3b_voxel_cfg* cfg, const float* points, int n_rows, int n_chunks,
-                           float* voxels, int32_t* coors, int32_t* num_points, float* mean_feats, int32_t* voxel_counts,
+// The grid-stride kernels are sized for the capacity's rows and the rank-chunk grids for its chunks plus one partial
+// chunk per cloud; the kernels stop at the live counts they read from the offsets.
+static int launch_voxelize(const VoxParams& p, const d3b_voxel_cfg* cfg, const float* points, float* voxels,
+                           int32_t* coors, int32_t* num_points, float* mean_feats, int32_t* voxel_counts,
                            int32_t* status, const VoxWorkspace& w, cudaStream_t stream) {
+  const int n_rows = p.point_cap, n_chunks = div_up(p.point_cap, kRankChunk) + p.batch;
   D3B_CUDA(cudaMemsetAsync(w.keys, 0xff, w.cap * 8, stream));
   D3B_CUDA(cudaMemsetAsync(w.first, 0x7f, w.sentinel_bytes, stream));
   if (n_rows > 0) {
@@ -444,16 +418,12 @@ static int launch_voxelize(const VoxParams& p, const d3b_voxel_cfg* cfg, const f
                                                            (unsigned int)(w.cap - 1));
     D3B_LAUNCH_CHECK();
   }
-  if (n_chunks > 0) {
-    vox_chunk_count<<<n_chunks, 256, 0, stream>>>(p, w.first, w.pslot, w.chunk_cnt);
-    D3B_LAUNCH_CHECK();
-  }
+  vox_chunk_count<<<n_chunks, 256, 0, stream>>>(p, w.first, w.pslot, w.chunk_cnt);
+  D3B_LAUNCH_CHECK();
   vox_chunk_scan<<<p.batch, 1024, 0, stream>>>(p, w.chunk_cnt, w.chunk_base, w.cut, voxel_counts, status);
   D3B_LAUNCH_CHECK();
-  if (n_chunks > 0) {
-    vox_assign<<<n_chunks, 256, 0, stream>>>(p, w.first, w.pslot, w.chunk_base, w.vid, w.vslot, w.cut);
-    D3B_LAUNCH_CHECK();
-  }
+  vox_assign<<<n_chunks, 256, 0, stream>>>(p, w.first, w.pslot, w.chunk_base, w.vid, w.vslot, w.cut);
+  D3B_LAUNCH_CHECK();
   if (n_rows > 0) {
     vox_lists<<<grid_for(n_rows, 256), 256, 0, stream>>>(p, w.pslot, w.vid, w.cut, w.lists);
     D3B_LAUNCH_CHECK();
@@ -466,44 +436,25 @@ static int launch_voxelize(const VoxParams& p, const d3b_voxel_cfg* cfg, const f
   return D3B_OK;
 }
 
-extern "C" int d3b_voxelize(const d3b_voxel_cfg* cfg, const float* points,
-                            const int32_t* cloud_offsets, int32_t batch, float* voxels,
-                            int32_t* coors, int32_t* num_points, float* mean_feats,
-                            int32_t* voxel_counts, void* workspace, size_t workspace_bytes,
-                            void* stream_) {
-  D3B_REQUIRE(cfg && cloud_offsets && coors && num_points && voxel_counts && workspace,
-              "d3b_voxelize: null argument");
-  const int st = check_cfg(cfg, batch, "d3b_voxelize");
-  if (st != D3B_OK) return st;
-  VoxParams p = params_of(cfg, batch);
-  for (int b = 0; b <= batch; ++b) {
-    p.off[b] = cloud_offsets[b];
-    D3B_REQUIRE(b == 0 ? p.off[b] == 0 : p.off[b] >= p.off[b - 1], "d3b_voxelize: cloud_offsets not monotone");
-    p.chunk_off[b] = b == 0 ? 0 : p.chunk_off[b - 1] + (p.off[b] - p.off[b - 1] + kRankChunk - 1) / kRankChunk;
-  }
-  const int n_total = p.off[batch];
-  D3B_REQUIRE(n_total == 0 || points, "d3b_voxelize: null points");
-  VoxWorkspace w = carve(cfg, n_total, batch, (char*)workspace);
-  if (w.bytes > workspace_bytes) {
-    set_error("d3b_voxelize: workspace %zu < %zu", workspace_bytes, w.bytes);
-    return D3B_ERR_WORKSPACE;
-  }
-  return launch_voxelize(p, cfg, points, n_total, p.chunk_off[batch], voxels, coors, num_points, mean_feats,
-                         voxel_counts, nullptr, w, (cudaStream_t)stream_);
-}
-
 extern "C" int d3b_voxelize_dev(const d3b_voxel_cfg* cfg, const float* points, int32_t point_capacity,
                                 const int32_t* cloud_offsets_dev, int32_t batch, float* voxels, int32_t* coors,
                                 int32_t* num_points, float* mean_feats, int32_t* voxel_counts, int32_t* status,
                                 void* workspace, size_t workspace_bytes, void* stream_) {
   D3B_REQUIRE(cfg && cloud_offsets_dev && coors && num_points && voxel_counts && workspace,
               "d3b_voxelize_dev: null argument");
-  const int st = check_cfg(cfg, batch, "d3b_voxelize_dev");
-  if (st != D3B_OK) return st;
+  D3B_REQUIRE(batch >= 1 && batch <= kMaxBatch, "d3b_voxelize_dev: batch %d outside [1,%d]", batch, kMaxBatch);
+  D3B_REQUIRE(cfg->ndim >= 3 && cfg->max_points >= 1 && cfg->max_voxels >= 1,
+              "d3b_voxelize_dev: bad cfg (ndim %d, max_points %d, max_voxels %d)", cfg->ndim, cfg->max_points,
+              cfg->max_voxels);
+  for (int j = 0; j < 3; ++j)
+    D3B_REQUIRE(cfg->grid[j] >= 1 && cfg->voxel_size[j] > 0.0f, "d3b_voxelize_dev: bad grid/voxel_size");
+  D3B_REQUIRE((double)cfg->grid[0] * cfg->grid[1] * cfg->grid[2] * batch < 9.0e18, "d3b_voxelize_dev: grid too large");
   D3B_REQUIRE(point_capacity >= 0 && point_capacity <= (1 << 30), "d3b_voxelize_dev: point_capacity %d outside [0, 2^30]",
               point_capacity);
   D3B_REQUIRE(point_capacity == 0 || points, "d3b_voxelize_dev: null points");
-  VoxParams p = params_of(cfg, batch);
+  VoxParams p;
+  for (int j = 0; j < 3; ++j) { p.vs[j] = cfg->voxel_size[j]; p.lo[j] = cfg->range_min[j]; p.grid[j] = cfg->grid[j]; }
+  p.ndim = cfg->ndim; p.max_points = cfg->max_points; p.max_voxels = cfg->max_voxels; p.batch = batch;
   p.off_dev = cloud_offsets_dev;
   p.point_cap = point_capacity;
   VoxWorkspace w = carve(cfg, point_capacity, batch, (char*)workspace);
@@ -511,6 +462,6 @@ extern "C" int d3b_voxelize_dev(const d3b_voxel_cfg* cfg, const float* points, i
     set_error("d3b_voxelize_dev: workspace %zu < %zu", workspace_bytes, w.bytes);
     return D3B_ERR_WORKSPACE;
   }
-  return launch_voxelize(p, cfg, points, point_capacity, div_up(point_capacity, kRankChunk) + batch, voxels, coors,
-                         num_points, mean_feats, voxel_counts, status, w, (cudaStream_t)stream_);
+  return launch_voxelize(p, cfg, points, voxels, coors, num_points, mean_feats, voxel_counts, status, w,
+                         (cudaStream_t)stream_);
 }

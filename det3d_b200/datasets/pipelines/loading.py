@@ -1,6 +1,6 @@
 """On-disk -> device ingest (SURVEY 8f.4): `LoadPointCloudFromFile` with the reference's registry name, constructor
 and `__call__(res, info)` contract (det3d/datasets/pipelines/loading.py:67-124), the NuScenes multi-sweep merge done
-on the GPU by d3b_ingest_sweeps (csrc/ingest.cu).
+on the GPU by d3b_ingest_sweeps_dev (csrc/ingest.cu).
 
 File reading stays on the host (it is I/O): KITTI `.bin` = flat float32 [N, num_point_features] (:92-94), nuScenes
 and Lyft `.bin` = float32 [N, 5] of which the first 4 columns are kept (`read_file`, :17-31; Lyft reads the
@@ -11,12 +11,12 @@ numpy fields as the reference (`points`, `times`, `combined`) plus `combined_cud
 voxelizer consumes directly (no second H2D copy).
 
 `ingest_sweeps_batched` does the same for a batch of samples in one d3b_ingest_sweeps_dev call: the sweep table lives
-in device memory and the per-sample cloud offsets stay there, in the form the voxelizer's device-offset path takes, so
-nothing between the raw sweeps and the detections waits on the host (InferencePipeline.infer_sweeps).
+in device memory and the per-sample cloud offsets stay there, in the form the voxelizer takes, so nothing between the
+raw sweeps and the detections waits on the host (InferencePipeline.infer_sweeps).  `ingest_sweeps` is a batch of one.
 
-`BatchedIngest(gather=True)` runs d3b_ingest_sweeps_gather instead: the table also says at which raw row each sweep
-starts, so sweeps are read where they already lie in device memory (the history slots of apis.SweepStream), and
-`stream_transforms` gives the float64 key-frame transforms and lags of such a history.
+With `BatchedIngest(gather=True)` the table also says at which raw row each sweep starts (sweep_src), so sweeps are
+read where they already lie in device memory (the history slots of apis.SweepStream), and `stream_transforms` gives the
+float64 key-frame transforms and lags of such a history.
 """
 import collections
 import ctypes as C
@@ -27,6 +27,7 @@ import numpy as np
 import torch
 
 from ... import _lib
+from ...utils.staging import RowStager
 from ..registry import PIPELINES
 
 
@@ -53,36 +54,10 @@ def read_file(path, tries=2, num_point_feature=4, keep_raw=False):
 def ingest_sweeps(raw_sweeps, transforms, time_lags, radius=1.0, n_feat=4, device="cuda"):
     """raw_sweeps: list of float32 [n_s, 5] arrays, key frame first.  transforms[s]: 4x4 array or None;
     time_lags[s]: float.  The key frame (s = 0) is neither filtered nor transformed, as in the reference.
-    Returns the device tensor [N, n_feat + 1] (x, y, z, .., time lag), input order preserved."""
-    if not torch.cuda.is_available():
-        raise RuntimeError("det3d_b200: the multi-sweep ingest needs a CUDA device (there is no CPU fallback)")
-    n_sweeps = len(raw_sweeps)
-    sizes = [int(r.shape[0]) for r in raw_sweeps]
-    offsets = (C.c_int32 * (n_sweeps + 1))(*np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64).tolist())
-    n_total = int(sum(sizes))
-    dev = torch.device(device)
-    stride = int(raw_sweeps[0].shape[1]) if n_sweeps else 5
-    raw = torch.from_numpy(np.ascontiguousarray(np.concatenate(raw_sweeps, axis=0), dtype=np.float32)).to(dev)
-    tm = np.zeros((n_sweeps, 16), np.float64)
-    has = np.zeros(n_sweeps, np.uint8)
-    for s, t in enumerate(transforms):
-        if t is not None:
-            tm[s] = np.asarray(t, np.float64).reshape(16)
-            has[s] = 1
-    lag = np.asarray(time_lags, np.float64).astype(np.float32)       # times.astype(points.dtype), loading.py:119
-    filt = np.ones(n_sweeps, np.uint8)
-    filt[0] = 0
-    out = torch.empty((max(n_total, 1), n_feat + 1), dtype=torch.float32, device=dev)
-    n_out = torch.zeros(1, dtype=torch.int32, device=dev)
-    ws = torch.empty(_lib.lib().d3b_ingest_workspace_bytes(n_total), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        st = _lib.lib().d3b_ingest_sweeps(
-            raw.data_ptr(), offsets, n_sweeps, stride, n_feat, tm.ctypes.data, has.ctypes.data, lag.ctypes.data,
-            filt.ctypes.data, C.c_float(radius), out.data_ptr(), n_total, n_out.data_ptr(), ws.data_ptr(), ws.numel(),
-            _lib.current_stream())
-        _lib.check(st, "d3b_ingest_sweeps")
-        n = int(n_out.item())            # API boundary: the reference returns exactly-sized arrays
-    return out[:n]
+    Returns the device tensor [N, n_feat + 1] (x, y, z, .., time lag), input order preserved: ingest_sweeps_batched on
+    a batch of one, cut to its exact length (one sync)."""
+    points, offsets = ingest_sweeps_batched([(raw_sweeps, transforms, time_lags)], radius, n_feat, device)
+    return points[:int(offsets[1])]              # API boundary: the reference returns exactly-sized arrays
 
 
 MAX_SWEEPS = 16          # D3B_INGEST_MAX_SWEEPS: sweeps per sample, key frame included
@@ -266,41 +241,6 @@ class SweepHistory:
         return out
 
 
-class RowStager:
-    """H2D copies of host row arrays into device rows.  Pinned tensors are copied directly; anything else goes through
-    a pinned staging buffer shaped like the device rows, allocated on first need.  The staging buffer may still feed
-    the previous put's copies when the next put rewrites it, so each put waits for those first (its own event)."""
-
-    def __init__(self):
-        self.staging = None
-        self.copied = None
-
-    def put(self, arrays, dst):
-        """Enqueues the H2D copies of `arrays` (float32 [n_i, dst.shape[1]] host arrays or tensors) back to back into
-        the device rows dst[0:sum(n_i)]; every put of one stager has dst of the same shape.  Returns sum(n_i)."""
-        at, staged = 0, False
-        with torch.cuda.device(dst.device):
-            for a in arrays:
-                k = int(a.shape[0])
-                if not k:
-                    continue
-                src = a
-                if not (torch.is_tensor(a) and a.is_pinned()):
-                    if self.staging is None:
-                        self.staging = torch.empty(dst.shape, dtype=torch.float32, pin_memory=True)
-                        self.copied = torch.cuda.Event()
-                    if not staged:
-                        self.copied.synchronize()
-                        staged = True
-                    src = self.staging[at:at + k]
-                    src.copy_(torch.as_tensor(a))
-                dst[at:at + k].copy_(src, non_blocking=True)
-                at += k
-            if staged:
-                self.copied.record()
-        return at
-
-
 def stage_raw_sweeps(samples, sizes, raw_dev):
     """Enqueues the H2D copies of every raw sweep into raw_dev, back to back in sample order, through a RowStager of
     its own.  `sizes` (check_sweep_samples') is not read: each array's shape gives its rows.  Returns the number of
@@ -312,7 +252,7 @@ class BatchedIngest:
     """Device buffers of one batched-ingest shape -- raw [raw_capacity, raw_stride], the sweep table, the ingested
     clouds [raw_capacity, n_feat + 1], cloud_offsets [B + 1], status, workspace -- and the d3b_ingest_sweeps_dev call
     over them.  The addresses never change, so a captured CUDA graph can hold them.  With `gather` the table also holds
-    sweep_src (the raw row where each sweep starts) and launch() runs d3b_ingest_sweeps_gather."""
+    sweep_src (the raw row where each sweep starts), which launch() passes; without it each sweep starts at its offset."""
 
     def __init__(self, batch, raw_capacity, sweep_capacity, raw_stride, n_feat=4, radius=1.0, device="cuda",
                  gather=False):
@@ -345,16 +285,14 @@ class BatchedIngest:
     def launch(self):
         """Ingests the raw sweeps under the device table into out / cloud_offsets (three kernels, no host sync)."""
         t = self.tables
-        L, name = _lib.lib(), "d3b_ingest_sweeps_gather" if self.gather else "d3b_ingest_sweeps_dev"
-        head = (self.raw.data_ptr(), self.raw_capacity, self.raw_stride, self.n_feat, t["sweep_offsets"].data_ptr())
-        head += (t["sweep_src"].data_ptr(),) if self.gather else ()
         with _lib.on_device_of(self.raw), _lib.timed("ingest_sweeps", batch=self.batch, capacity=self.raw_capacity):
-            st = getattr(L, name)(
-                *head, t["sample_sweeps"].data_ptr(), t["transforms"].data_ptr(), t["time_lag"].data_ptr(),
-                t["flags"].data_ptr(), self.sweep_capacity, self.batch, C.c_float(self.radius), self.out.data_ptr(),
-                self.cloud_offsets.data_ptr(), self.status.data_ptr(), self.ws.data_ptr(), self.ws.numel(),
-                _lib.current_stream())
-        _lib.check(st, name)
+            st = _lib.lib().d3b_ingest_sweeps_dev(
+                self.raw.data_ptr(), self.raw_capacity, self.raw_stride, self.n_feat, t["sweep_offsets"].data_ptr(),
+                _lib.ptr(t.get("sweep_src")), t["sample_sweeps"].data_ptr(), t["transforms"].data_ptr(),
+                t["time_lag"].data_ptr(), t["flags"].data_ptr(), self.sweep_capacity, self.batch, C.c_float(self.radius),
+                self.out.data_ptr(), self.cloud_offsets.data_ptr(), self.status.data_ptr(), self.ws.data_ptr(),
+                self.ws.numel(), _lib.current_stream())
+        _lib.check(st, "d3b_ingest_sweeps_dev")
         return self.out, self.cloud_offsets
 
 
@@ -362,7 +300,7 @@ def ingest_sweeps_batched(samples, radius=1.0, n_feat=4, device="cuda", capacity
     """Batched ingest_sweeps: samples = [(raw_sweeps, transforms, time_lags), ...], each with ingest_sweeps' contract
     (key frame first; it is neither filtered nor transformed unless a transform is given).  One d3b_ingest_sweeps_dev
     call, no host sync.  Returns (points [capacity, n_feat + 1], cloud_offsets int32 [B + 1]), both on the device:
-    sample b's cloud is points[cloud_offsets[b]:cloud_offsets[b + 1]], bit-identical to ingest_sweeps on that sample;
+    sample b's cloud is points[cloud_offsets[b]:cloud_offsets[b + 1]], the bits that sample gives alone (ingest_sweeps);
     rows past cloud_offsets[B] are undefined.  capacity (default: the raw total) must be >= the raw total."""
     if not torch.cuda.is_available():
         raise RuntimeError("det3d_b200: the multi-sweep ingest needs a CUDA device (there is no CPU fallback)")

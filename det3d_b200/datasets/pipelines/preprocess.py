@@ -4,10 +4,10 @@
 Same constructor keywords and the same `__call__(res, info) -> (res, info)` contract, so the `test_pipeline` of an
 unmodified Det3D config builds through `PIPELINES`.  What changes is where the work runs:
 
-* `Voxelization` calls `VoxelGenerator.generate`, i.e. d3b_voxelize on the GPU (csrc/voxelize.cu), and fills
+* `Voxelization` calls `VoxelGenerator.generate`, i.e. d3b_voxelize_dev on the GPU (csrc/voxelize.cu), and fills
   `res["lidar"]["voxels"]` with exactly the reference's dict (`voxels, coordinates, num_points, num_voxels [1] int64,
-  shape`).  `Voxelization.batched(points_list)` is the fused front the serving path uses: ONE d3b_voxelize call for the
-  whole batch with the batch index (collate_kitti, collate.py:130-137) and the VFE mean already applied, outputs on the
+  shape`).  `Voxelization.batched(points_list)` is the fused front the serving path uses: ONE d3b_voxelize_dev call for
+  the whole batch with the batch index (collate_kitti, collate.py:130-137) and the VFE mean already applied, outputs on the
   device.
 * `AssignTarget` in val/test mode only produces `anchors` (the reference regenerates them on the CPU for every sample,
   preprocess.py:355-378); here they are generated once per feature-map size and cached.
@@ -120,7 +120,7 @@ class Voxelization(object):
         return res, info
 
     def batched(self, points_list, device="cuda", want_voxels=True, want_mean=True):
-        """Voxelization + collate_kitti for a whole batch in ONE d3b_voxelize call (SURVEY 8f.1).
+        """Voxelization + collate_kitti for a whole batch in ONE d3b_voxelize_dev call (SURVEY 8f.1).
 
         points_list: per-sample float32 [N_i, ndim] arrays / tensors (host or device).  Returns device tensors with
         the collated layout: voxels [M, max_points, ndim] (optional), coordinates [M, 4] (b, z, y, x), num_points [M],

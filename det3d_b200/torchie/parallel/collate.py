@@ -8,7 +8,7 @@ Two forms:
   are concatenated (:101-102), `anchors` are stacked per task (:138-147), `metadata` stays a list, `calib` is stacked
   per key, everything else is `np.stack`ed.  Pure host glue, written against the same key table.
 * `collate_kitti_device(points_list, voxelization)` -- the fused form the serving path uses (SURVEY 8f.1): raw clouds ->
-  the SAME batch dict, produced by one batched d3b_voxelize call (batch index written by the kernel, outputs resident
+  the SAME batch dict, produced by one batched d3b_voxelize_dev call (batch index written by the kernel, outputs resident
   on the GPU), so the `[M, max_points, ndim]` host tensors and their H2D copy never exist.
 
 Training-only keys (`gt_boxes`, `labels`, `reg_targets`, ...) raise: target assignment is out of scope.

@@ -68,88 +68,59 @@ typedef struct {
 size_t d3b_voxelize_workspace_bytes(const d3b_voxel_cfg* cfg, int32_t n_points_total,
                                     int32_t batch);
 
-/* points        [n_total, ndim] f32 device, clouds concatenated
- * cloud_offsets [batch + 1] i32 HOST: cloud b owns points [off[b], off[b+1])
- * voxels        [batch*max_voxels, max_points, ndim] f32 device, or NULL
- * coors         [batch*max_voxels, 4] i32 device (batch, z, y, x)
- * num_points    [batch*max_voxels] i32 device
- * mean_feats    [batch*max_voxels, ndim] f32 device, or NULL
- * voxel_counts  [batch + 1] i32 device: [b] = voxels of cloud b, [batch] = total.
- * Rows of all clouds are written back to back (cloud 0 first); only the
- * first voxel_counts[batch] rows of each output are defined. */
-int d3b_voxelize(const d3b_voxel_cfg* cfg, const float* points, const int32_t* cloud_offsets,
-                 int32_t batch, float* voxels, int32_t* coors, int32_t* num_points,
-                 float* mean_feats, int32_t* voxel_counts, void* workspace,
-                 size_t workspace_bytes, void* stream);
-
-/* d3b_voxelize with the cloud offsets in DEVICE memory, for graph replay over clouds of any size.
- * points            [point_capacity, ndim] f32 device; rows at or past off[batch] are never read
- * cloud_offsets_dev [batch + 1] i32 DEVICE
+/* Voxelizes `batch` clouds in one call, with the cloud offsets in DEVICE memory, so one captured CUDA graph serves clouds
+ * of any size up to point_capacity.
+ * points            [point_capacity, ndim] f32 device, clouds concatenated; rows at or past off[batch] are never read
+ * cloud_offsets_dev [batch + 1] i32 DEVICE: cloud b owns points [off[b], off[b+1])
+ * voxels            [batch*max_voxels, max_points, ndim] f32 device, or NULL
+ * coors             [batch*max_voxels, 4] i32 device (batch, z, y, x)
+ * num_points        [batch*max_voxels] i32 device
+ * mean_feats        [batch*max_voxels, ndim] f32 device, or NULL
+ * voxel_counts      [batch + 1] i32 device: [b] = voxels of cloud b, [batch] = total.
  * status            [1] i32 device or NULL: set to 1 if the offsets were not 0 = off[0] <= ... <= off[batch] <= point_capacity;
  *                   they are then clamped into that shape before any point index is formed (0 when they were)
  * workspace: d3b_voxelize_workspace_bytes(cfg, point_capacity, batch); point lists: d3b_voxelize_point_lists(cfg, point_capacity, batch, ws)
- * Outputs are bit-identical to d3b_voxelize's on the same clouds, for any capacity >= off[batch]. */
+ * Rows of all clouds are written back to back (cloud 0 first); only the first voxel_counts[batch] rows of each output
+ * are defined.  The outputs are the same bits for any capacity >= off[batch]. */
 int d3b_voxelize_dev(const d3b_voxel_cfg* cfg, const float* points, int32_t point_capacity,
                      const int32_t* cloud_offsets_dev, int32_t batch, float* voxels, int32_t* coors,
                      int32_t* num_points, float* mean_feats, int32_t* voxel_counts, int32_t* status,
                      void* workspace, size_t workspace_bytes, void* stream);
 
-/* Multi-sweep ingest (nuScenes): raw sweeps of one sample -> one cloud [n, n_feat + 1] = (x, y, z, .., time lag).
+/* Multi-sweep ingest (nuScenes) for a batch of samples: each sample's raw sweeps -> one cloud [n, n_feat + 1] =
+ * (x, y, z, .., time lag), with the sweep table in DEVICE memory, for graph replay over sweeps of any size.
  * replaces read_file / remove_close / read_sweep and the NuScenes branch of LoadPointCloudFromFile.__call__,
- * det3d/datasets/pipelines/loading.py:17-64,98-124.
- * raw            [n_total, raw_stride] f32 device: the sweeps' file contents back to back, key frame first
- * sweep_offsets  [n_sweeps + 1] i32 HOST, in points
- * transforms     [n_sweeps, 16] f64 HOST row-major 4x4 (read where has_transform[s]; may be NULL otherwise)
- * has_transform, filter_close [n_sweeps] u8 HOST, time_lag [n_sweeps] f32 HOST
- * filter_close[s]: drop points with |x| < radius and |y| < radius before the transform (remove_close)
- * out            [out_cap, n_feat + 1] f32 device, n_out [1] i32 device = min(kept points, out_cap); input order kept */
-#define D3B_INGEST_MAX_SWEEPS 16
-size_t d3b_ingest_workspace_bytes(int32_t n_points_total);
-int d3b_ingest_sweeps(const float* raw, const int32_t* sweep_offsets, int32_t n_sweeps, int32_t raw_stride,
-                      int32_t n_feat, const double* transforms, const uint8_t* has_transform, const float* time_lag,
-                      const uint8_t* filter_close, float radius, float* out, int32_t out_cap, int32_t* n_out,
-                      void* workspace, size_t workspace_bytes, void* stream);
-
-/* d3b_ingest_sweeps for a batch of samples with the sweep table in DEVICE memory, for graph replay over sweeps of any
- * size; runs the same three kernels, whatever the batch (no host sync).  S = sweep_capacity, 1 <= batch <= 64,
- * 1 <= S <= D3B_INGEST_MAX_SWEEPS * batch.
- * raw            [raw_capacity, raw_stride] f32 device: every sweep of every sample back to back, each sample's key frame
- *                first; rows at or past sweep_offsets[sample_sweeps[batch]] are never read
- * sweep_offsets  [S + 1] i32 DEVICE, raw rows: sweep s owns rows [sweep_offsets[s], sweep_offsets[s + 1])
+ * det3d/datasets/pipelines/loading.py:17-64,98-124.  Runs three kernels, whatever the batch (no host sync).
+ * S = sweep_capacity, 1 <= batch <= 64, 1 <= S <= D3B_INGEST_MAX_SWEEPS * batch.
+ * raw            [raw_capacity, raw_stride] f32 device: the sweeps' file contents, each sample's key frame first; rows no
+ *                sweep covers are never read
+ * sweep_offsets  [S + 1] i32 DEVICE: the logical prefix of the sweeps' lengths, len_s = sweep_offsets[s + 1] -
+ *                sweep_offsets[s]; it drives the chunking, the scan and cloud_offsets
+ * sweep_src      [S] i32 DEVICE or NULL: sweep s is rows [sweep_src[s], sweep_src[s] + len_s) of raw (e.g. a ring of
+ *                per-stream history slots that stay on the device from one frame to the next).  NULL: sweep s is rows
+ *                [sweep_offsets[s], sweep_offsets[s + 1]), the sweeps back to back; the same as sweep_src[s] =
+ *                sweep_offsets[s], bit for bit
  * sample_sweeps  [batch + 1] i32 DEVICE: sample b owns sweeps [sample_sweeps[b], sample_sweeps[b + 1])
  * transforms     [S, 16] f64 DEVICE row-major 4x4, time_lag [S] f32 DEVICE
- * flags          [S] u8 DEVICE: bit 0 = has_transform, bit 1 = filter_close (as d3b_ingest_sweeps; a key frame has neither)
+ * flags          [S] u8 DEVICE: bit 0 = has_transform, bit 1 = filter_close (drop points with |x| < radius and
+ *                |y| < radius before the transform: remove_close); a key frame has neither
  * out            [raw_capacity, n_feat + 1] f32 device: the samples' clouds back to back, each in input order
  * cloud_offsets  [batch + 1] i32 device: sample b's cloud is rows [cloud_offsets[b], cloud_offsets[b + 1]) of `out` --
  *                the form d3b_voxelize_dev takes
- * status         [1] i32 device or NULL: set to 1 if the tables were not 0 = sweep_offsets[0] <= ... <= sweep_offsets[S]
- *                <= raw_capacity and 0 = sample_sweeps[0] <= ... <= sample_sweeps[batch] <= S; they are then clamped
- *                into that shape as t[i] = min(max(0, t[1..i]), bound) before any point index is formed (0 when they were)
- * workspace: d3b_ingest_dev_workspace_bytes(raw_capacity, S).  Each sample's rows are bit-identical to d3b_ingest_sweeps's
- * output for that sample alone. */
+ * status         [1] i32 device or NULL.  Bit 0 (value 1) is set if the tables were not 0 = sweep_offsets[0] <= ... <=
+ *                sweep_offsets[S] <= raw_capacity and 0 = sample_sweeps[0] <= ... <= sample_sweeps[batch] <= S; they are
+ *                then clamped into that shape as t[i] = min(max(0, t[1..i]), bound) before any point index is formed.
+ *                After that, each sweep_src[s] is clamped into [0, raw_capacity - len_s], identically in every CTA,
+ *                and bit 1 (value 2) is set when that changed anything.  0 when nothing was clamped.
+ * workspace: d3b_ingest_dev_workspace_bytes(raw_capacity, S).  Each sample's rows are the bits it gives as a batch of
+ * one. */
+#define D3B_INGEST_MAX_SWEEPS 16
 size_t d3b_ingest_dev_workspace_bytes(int32_t raw_capacity, int32_t sweep_capacity);
 int d3b_ingest_sweeps_dev(const float* raw, int32_t raw_capacity, int32_t raw_stride, int32_t n_feat,
-                          const int32_t* sweep_offsets, const int32_t* sample_sweeps, const double* transforms,
-                          const float* time_lag, const uint8_t* flags, int32_t sweep_capacity, int32_t batch,
-                          float radius, float* out, int32_t* cloud_offsets, int32_t* status, void* workspace,
-                          size_t workspace_bytes, void* stream);
-
-/* d3b_ingest_sweeps_dev with each sweep read from wherever it lies in `raw` (e.g. a ring of per-stream history slots that
- * stay on the device from one frame to the next).  Same arguments, plus
- * sweep_src      [S] i32 DEVICE: sweep s is rows [sweep_src[s], sweep_src[s] + len_s) of raw, len_s = sweep_offsets[s + 1] -
- *                sweep_offsets[s]; rows no sweep covers are never read
- * sweep_offsets keeps its role as the logical prefix of the sweeps' lengths: it drives the chunking, the scan and
- * cloud_offsets, so `out` / cloud_offsets are laid out exactly as d3b_ingest_sweeps_dev's, and its bound is still
- * sweep_offsets[S] <= raw_capacity.  After the offsets are clamped, each sweep_src[s] is clamped into
- * [0, raw_capacity - len_s], identically in every CTA, before any point index is formed; status bit 1 (value 2) is set
- * when that changed anything, bit 0 (value 1) keeps its meaning.  With sweep_src[s] = sweep_offsets[s] the results are
- * d3b_ingest_sweeps_dev's, bit for bit.  workspace: d3b_ingest_gather_workspace_bytes(raw_capacity, S). */
-size_t d3b_ingest_gather_workspace_bytes(int32_t raw_capacity, int32_t sweep_capacity);
-int d3b_ingest_sweeps_gather(const float* raw, int32_t raw_capacity, int32_t raw_stride, int32_t n_feat,
-                             const int32_t* sweep_offsets, const int32_t* sweep_src, const int32_t* sample_sweeps,
-                             const double* transforms, const float* time_lag, const uint8_t* flags,
-                             int32_t sweep_capacity, int32_t batch, float radius, float* out, int32_t* cloud_offsets,
-                             int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+                          const int32_t* sweep_offsets, const int32_t* sweep_src, const int32_t* sample_sweeps,
+                          const double* transforms, const float* time_lag, const uint8_t* flags,
+                          int32_t sweep_capacity, int32_t batch, float radius, float* out, int32_t* cloud_offsets,
+                          int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
 
 /* KITTI camera-frustum crop for a batch of raw scans, with the cloud offsets and the planes in DEVICE memory, for graph
  * replay over scans of any size.  replaces box_np_ops.remove_outside_points (det3d/core/bbox/box_np_ops.py:941-952;
@@ -305,10 +276,10 @@ int d3b_pillar_features(const float* voxels, const int32_t* num_points, const in
                         float vx, float vy, float x_offset, float y_offset, float* out, void* stream);
 
 /* The same reader fused with the voxelizer (SURVEY 8f.3): the pillar's points are fetched through the voxelizer's
- * per-voxel point-index lists, so the [rows, max_points, ndim] voxel tensor is never materialised (call d3b_voxelize
- * with voxels = NULL).  `lists` = d3b_voxelize_point_lists(...) of the workspace that d3b_voxelize just filled:
+ * per-voxel point-index lists, so the [rows, max_points, ndim] voxel tensor is never materialised (call d3b_voxelize_dev
+ * with voxels = NULL).  `lists` = d3b_voxelize_point_lists(...) of the workspace that d3b_voxelize_dev just filled:
  * [batch][max_voxels][max_points] int32 indices into `points`, >= 0x7f000000 = empty slot; valid until that workspace is
- * used again.  voxel_counts = d3b_voxelize's per-cloud counts.  Everything else as d3b_pillar_features. */
+ * used again.  voxel_counts = d3b_voxelize_dev's per-cloud counts.  Everything else as d3b_pillar_features. */
 const int32_t* d3b_voxelize_point_lists(const d3b_voxel_cfg* cfg, int32_t n_points_total, int32_t batch, void* workspace);
 int d3b_pillar_features_lists(const float* points, const int32_t* lists, const int32_t* voxel_counts, int32_t batch,
                               int32_t max_voxels, const int32_t* num_points, const int32_t* coors, const int32_t* n_rows,

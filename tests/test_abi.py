@@ -56,13 +56,14 @@ def test_every_plane_writer_takes_an_overflow_flag():
     assert not missing, "write f16 planes without an overflow flag: %s" % missing
 
 
-def test_abi_4_and_error_string():
-    """ABI 4: the rulebook builders no longer take pair lists (three arguments fewer than in ABI 3), and
-    d3b_conv_params lost its pair-kernel fields."""
+def test_abi_5_and_error_string():
+    """ABI 5: the voxelizer and the sweep ingest take their tables from device memory only (d3b_voxelize_dev,
+    d3b_ingest_sweeps_dev with a nullable sweep_src); since ABI 4 the rulebook builders take no pair lists."""
     L = _lib.lib()
-    assert L.d3b_abi_version() == 4
+    assert L.d3b_abi_version() == 5
     assert len(_lib.SIGNATURES["d3b_rulebook_subm"][1]) == 8
     assert len(_lib.SIGNATURES["d3b_rulebook_conv"][1]) == 16
+    assert len(_lib.SIGNATURES["d3b_ingest_sweeps_dev"][1]) == 19
     assert isinstance(L.d3b_last_error(), bytes)
     assert L.d3b_launch_count() >= 0
 
@@ -73,9 +74,10 @@ def test_argument_validation_without_gpu():
     assert L.d3b_voxelize_workspace_bytes(None, 10, 1) == 0
     st = L.d3b_sparse_conv(None, None, None, None, 10, None, None, None)
     assert st == 1 and b"null" in L.d3b_last_error()
-    cfg = _lib.VoxelCfg()
-    st = L.d3b_voxelize(ctypes.byref(cfg), None, None, 1, None, None, None, None, None, None, 0, None)
-    assert st == 1
+    cfg = _lib.VoxelCfg()                                   # all zero: no grid, ndim 0
+    dummy = (ctypes.c_int32 * 2)()
+    st = L.d3b_voxelize_dev(ctypes.byref(cfg), None, 0, dummy, 1, None, dummy, dummy, None, dummy, None, dummy, 0, None)
+    assert st == 1 and b"cfg" in L.d3b_last_error()
 
 
 def test_sparse_conv_rejects_an_unknown_algo_without_gpu():
@@ -111,11 +113,15 @@ def test_entry_points_validate_before_cuda_without_gpu():
     off = (ctypes.c_int32 * 2)(0, 5)
     u8 = (ctypes.c_uint8 * 1)(0)
     lag = (ctypes.c_float * 1)(0.0)
-    n_out = (ctypes.c_int32 * 1)()
-    assert L.d3b_ingest_sweeps(None, off, 40, 5, 4, None, u8, lag, u8, 1.0, None, 5, n_out, None, 0, None) == 1
-    assert b"sweeps" in L.d3b_last_error()
-    assert L.d3b_ingest_sweeps(None, off, 1, 3, 4, None, u8, lag, u8, 1.0, None, 5, n_out, None, 0, None) == 1
-    assert L.d3b_ingest_workspace_bytes(-1) == 0 and L.d3b_nms_workspace_bytes(0) == 16
+    cloud = (ctypes.c_int32 * 2)()
+    # 40 sweeps for one sample, then raw_stride 3 < n_feat 4
+    assert L.d3b_ingest_sweeps_dev(None, 5, 5, 4, off, None, off, lag, lag, u8, 40, 1, 1.0, None, cloud, None, cloud,
+                                   1 << 20, None) == 1
+    assert b"sweep_capacity 40" in L.d3b_last_error()
+    assert L.d3b_ingest_sweeps_dev(None, 5, 3, 4, off, None, off, lag, lag, u8, 1, 1, 1.0, None, cloud, None, cloud, 1 << 20,
+                                   None) == 1
+    assert b"bad layout" in L.d3b_last_error()
+    assert L.d3b_ingest_dev_workspace_bytes(-1, 1) == 0 and L.d3b_nms_workspace_bytes(0) == 16
     q = _lib.PredictParams()
     assert L.d3b_predict_workspace_bytes(ctypes.byref(q)) == 0
     assert L.d3b_predict_task(ctypes.byref(q), None, 0, 0, None, None, 0, None) == 1

@@ -1,5 +1,5 @@
 """d3b_ingest_sweeps_dev and InferencePipeline.infer_sweeps validate their arguments on the host before any CUDA call
-(no GPU needed): status 1 (4 for a short workspace, as d3b_ingest_sweeps) with a message, and ValueError."""
+(no GPU needed): status 1 (4 for a short workspace) with a message, and ValueError."""
 import numpy as np
 import pytest
 import torch
@@ -15,8 +15,8 @@ def _call(raw=_P, capacity=4096, stride=5, n_feat=4, off=_P, samples=_P, tms=_P,
     L = _lib.lib()
     if ws_bytes is None:
         ws_bytes = L.d3b_ingest_dev_workspace_bytes(max(capacity, 0), max(table_cap, 1))
-    return L.d3b_ingest_sweeps_dev(raw, capacity, stride, n_feat, off, samples, tms, lags, flags, table_cap, batch, 1.0,
-                                   out, cloud_offsets, None, ws, ws_bytes, None)
+    return L.d3b_ingest_sweeps_dev(raw, capacity, stride, n_feat, off, None, samples, tms, lags, flags, table_cap, batch,
+                                   1.0, out, cloud_offsets, None, ws, ws_bytes, None)
 
 
 def test_null_arguments_are_rejected():
@@ -53,7 +53,7 @@ def test_small_workspace_is_rejected():
     L = _lib.lib()
     need = L.d3b_ingest_dev_workspace_bytes(4096, 8)
     assert need > 0
-    assert _call(ws_bytes=need - 1) == 4                              # D3B_ERR_WORKSPACE, as d3b_ingest_sweeps returns
+    assert _call(ws_bytes=need - 1) == 4                              # D3B_ERR_WORKSPACE
     assert b"workspace" in L.d3b_last_error()
 
 

@@ -1,7 +1,8 @@
 """Batched multi-sweep ingest with a device sweep table (d3b_ingest_sweeps_dev, ingest_sweeps_batched,
-InferencePipeline.infer_sweeps): every sample's rows are the bits d3b_ingest_sweeps gives for that sample alone, one
-captured graph serves tables of any size, malformed device tables are clamped and reported, and detections from raw
-sweeps equal the per-sample ingest followed by infer_host, for the CBGS and nuScenes PointPillars configs."""
+InferencePipeline.infer_sweeps): every sample's rows are the bits that sample gives as a batch of one (ingest_sweeps;
+its values are pinned by the reference golden in test_ingest.py), one captured graph serves tables of any size,
+malformed device tables are clamped and reported, and detections from raw sweeps equal the per-sample ingest followed
+by infer_host, for the CBGS and nuScenes PointPillars configs."""
 import argparse
 import os
 import warnings
@@ -29,6 +30,7 @@ def _golden_sample():
 
 
 def _per_sample(samples):
+    """Each sample ingested as a batch of one, cut to its rows."""
     from det3d.datasets.pipelines.loading import ingest_sweeps
     return [ingest_sweeps(*s) for s in samples]
 

@@ -1,5 +1,6 @@
-"""d3b_ingest_sweeps_gather and SweepStream without a GPU: the entry point's host-side argument checks, push()'s
-ValueErrors, and the slot bookkeeping, transforms and lags a stream computes on the host, against numpy."""
+"""The gather form of d3b_ingest_sweeps_dev (a non-null sweep_src) and SweepStream without a GPU: the entry point's
+host-side argument checks, push()'s ValueErrors, and the slot bookkeeping, transforms and lags a stream computes on the
+host, against numpy."""
 import numpy as np
 import pytest
 import torch
@@ -14,16 +15,16 @@ def _call(raw=_P, capacity=4096, stride=5, n_feat=4, off=_P, src=_P, samples=_P,
           table_cap=8, batch=2, out=_P, cloud_offsets=_P, ws=_P, ws_bytes=None):
     L = _lib.lib()
     if ws_bytes is None:
-        ws_bytes = L.d3b_ingest_gather_workspace_bytes(max(capacity, 0), max(table_cap, 1))
-    return L.d3b_ingest_sweeps_gather(raw, capacity, stride, n_feat, off, src, samples, tms, lags, flags, table_cap,
-                                      batch, 1.0, out, cloud_offsets, None, ws, ws_bytes, None)
+        ws_bytes = L.d3b_ingest_dev_workspace_bytes(max(capacity, 0), max(table_cap, 1))
+    return L.d3b_ingest_sweeps_dev(raw, capacity, stride, n_feat, off, src, samples, tms, lags, flags, table_cap, batch,
+                                   1.0, out, cloud_offsets, None, ws, ws_bytes, None)
 
 
 def test_gather_null_arguments_are_rejected():
     L = _lib.lib()
-    for name in ("off", "src", "samples", "tms", "lags", "flags", "cloud_offsets", "ws"):
+    for name in ("off", "samples", "tms", "lags", "flags", "cloud_offsets", "ws"):
         assert _call(**{name: None}) == 1, name
-        assert b"null" in L.d3b_last_error() and b"d3b_ingest_sweeps_gather" in L.d3b_last_error(), name
+        assert b"null" in L.d3b_last_error() and b"d3b_ingest_sweeps_dev" in L.d3b_last_error(), name
     for name in ("raw", "out"):
         assert _call(**{name: None}) == 1, name
         assert b"null buffer" in L.d3b_last_error(), name
@@ -47,9 +48,7 @@ def test_gather_bounds_and_layout_are_checked():
 
 def test_gather_workspace():
     L = _lib.lib()
-    for cap, S in ((0, 1), (4096, 8), (1 << 20, 64), (-1, 4), (100, 0)):
-        assert L.d3b_ingest_gather_workspace_bytes(cap, S) == L.d3b_ingest_dev_workspace_bytes(cap, S)
-    need = L.d3b_ingest_gather_workspace_bytes(4096, 8)
+    need = L.d3b_ingest_dev_workspace_bytes(4096, 8)
     assert _call(ws_bytes=need - 1) == 4                              # D3B_ERR_WORKSPACE
     assert b"workspace" in L.d3b_last_error()
 

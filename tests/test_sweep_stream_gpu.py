@@ -1,7 +1,8 @@
-"""Device-resident sweep histories (d3b_ingest_sweeps_gather, SweepStream): the gather ingest over sweeps scattered
-through a slot buffer gives the bits d3b_ingest_sweeps_dev gives over the same sweeps packed back to back, malformed
-sweep starts are clamped and reported, and every frame of a stream -- eager and graphed -- is bit-identical to
-infer_sweeps(stream.samples()), for the CBGS and nuScenes PointPillars configs, with one captured graph per sequence."""
+"""Device-resident sweep histories (d3b_ingest_sweeps_dev with a sweep_src table, SweepStream): the gather ingest over
+sweeps scattered through a slot buffer gives the bits the ingest without sweep_src gives over the same sweeps packed
+back to back, malformed sweep starts are clamped and reported, and every frame of a stream -- eager and graphed -- is
+bit-identical to infer_sweeps(stream.samples()), for the CBGS and nuScenes PointPillars configs, with one captured graph
+per sequence."""
 import warnings
 
 import numpy as np
@@ -100,6 +101,7 @@ def test_golden_sample_gathered():
 
 
 def test_sweep_src_at_the_offsets_is_the_dev_ingest():
+    """A null sweep_src and sweep_src[s] = sweep_offsets[s] give the same bits."""
     from det3d_b200.datasets.pipelines.loading import BatchedIngest, check_sweep_samples, stage_raw_sweeps
     samples = _mixed(6, 21)
     S = _table_cap(samples)

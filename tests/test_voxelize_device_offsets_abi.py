@@ -1,6 +1,9 @@
 """d3b_voxelize_dev validates its arguments on the host before any CUDA call (no GPU needed): status 1 (4 for a short
-workspace, as d3b_voxelize) and a message."""
+workspace) and a message; the Voxelizer rejects malformed host offsets before anything is allocated or enqueued."""
 import ctypes
+
+import pytest
+import torch
 
 from det3d_b200 import _lib
 
@@ -53,5 +56,15 @@ def test_small_workspace_is_rejected():
     cfg = _cfg()
     need = L.d3b_voxelize_workspace_bytes(ctypes.byref(cfg), 2048, 2)
     assert need > 0
-    assert _call(cfg, ws_bytes=need - 1) == 4                          # D3B_ERR_WORKSPACE, as d3b_voxelize returns
+    assert _call(cfg, ws_bytes=need - 1) == 4                          # D3B_ERR_WORKSPACE
     assert b"workspace" in L.d3b_last_error()
+
+
+@pytest.mark.parametrize("offsets", [[5, 10], [0, 7, 3, 10], [0, 4, 11], [0, 10, 10, 11], [0], [0] * 66, [-1, 10]])
+def test_voxelizer_rejects_malformed_host_offsets(offsets):
+    """off[0] != 0, decreasing, past the 10 rows of points (which would read past the buffer), batch 0 or 65."""
+    from det3d_b200.ops.point_cloud.voxelize import Voxelizer
+    vox = Voxelizer([0.05, 0.05, 0.1], [0, -40.0, -3.0, 70.4, 40.0, 1.0], 5, 100)
+    with pytest.raises(_lib.D3BError, match="Voxelizer"):
+        vox(torch.zeros((10, 4)), offsets)
+    assert vox._bufs == {}                                              # nothing allocated, nothing enqueued

@@ -1,6 +1,8 @@
-"""d3b_voxelize_dev (cloud offsets in device memory) against d3b_voxelize (host offsets): bit for bit on every output
-and on the per-voxel point-index lists, for any point capacity >= the live total, inside a CUDA graph replayed over
-offsets of different sizes, and with malformed offsets (flagged in `status`, then run clamped)."""
+"""d3b_voxelize_dev (cloud offsets in device memory) at any point capacity >= the live total against the same call at
+exactly the live total (the values themselves are pinned by the reference goldens: test_voxelize_gpu.py,
+test_oracle_voxel.py): bit for bit on every output and on the per-voxel point-index lists, with NaN / huge padding past
+the total, through the Voxelizer's host-offsets call, inside a CUDA graph replayed over offsets of different sizes, and
+with malformed offsets (flagged in `status`, then run clamped)."""
 import numpy as np
 import pytest
 import torch
@@ -47,13 +49,15 @@ def _assert_same(a, b):
 
 
 def _host(vox, clouds):
+    """The clouds through the Voxelizer's host-offsets call."""
     offs = np.cumsum([0] + [c.shape[0] for c in clouds]).tolist()
     pts = torch.from_numpy(np.concatenate(clouds).astype(np.float32)).cuda()
     return _result(vox, vox(pts, offs), len(clouds))
 
 
 def _dev(vox, clouds, capacity=None, pad=np.nan):
-    """The same clouds through d3b_voxelize_dev, rows past the live total filled with `pad`."""
+    """The clouds through d3b_voxelize_dev at `capacity` (default: exactly their total), rows past the live total
+    filled with `pad`."""
     offs = np.cumsum([0] + [c.shape[0] for c in clouds])
     total = int(offs[-1])
     capacity = total if capacity is None else capacity
@@ -70,10 +74,9 @@ def _dev(vox, clouds, capacity=None, pad=np.nan):
 def test_golden_cases_match_the_host_offsets_call(case):
     g = load_golden("voxel_" + case)
     vox = _voxelizer(g["voxel_size"], g["pcr"], int(g["max_points"]), int(g["max_voxels"]))
-    want = _host(vox, [g["points"]])
+    want = _dev(vox, [g["points"]])
     n = g["points"].shape[0]
-    if n > 0:
-        _assert_same(_dev(vox, [g["points"]]), want)
+    _assert_same(_host(vox, [g["points"]]), want)
     for capacity, pad in ((n + 1, np.nan), (n + 5000, 1e30), (4 * n + 1024, np.nan)):
         _assert_same(_dev(vox, [g["points"]], capacity, pad), want)
 
@@ -91,10 +94,10 @@ def test_mixed_batch_with_a_max_voxels_cut(want_voxels, want_mean):
     `break`)."""
     clouds = _mixed_clouds()
     vox = _voxelizer(KITTI["vs"], KITTI["pcr"], 5, 2500, want_voxels, want_mean)
-    want = _host(vox, clouds)
+    want = _dev(vox, clouds)
     assert want["counts"][3] == 2500 and want["counts"][1] == 0 and want["counts"][2] <= 1
     total = sum(c.shape[0] for c in clouds)
-    _assert_same(_dev(vox, clouds), want)
+    _assert_same(_host(vox, clouds), want)
     _assert_same(_dev(vox, clouds, total + 3000, np.nan), want)
     _assert_same(_dev(vox, clouds, 1 << 16, 1e30), want)
 
@@ -104,22 +107,22 @@ def test_batch_1_and_batch_64(want_voxels, want_mean):
     from det3d_b200.utils.synthetic import lidar_like_cloud
     vox = _voxelizer(KITTI["vs"], KITTI["pcr"], 5, 20000, want_voxels, want_mean)
     one = [lidar_like_cloud(20000, KITTI["pcr"], 4, 7)]
-    _assert_same(_dev(vox, one, 32768, 1e30), _host(vox, one))
+    _assert_same(_dev(vox, one, 32768, 1e30), _dev(vox, one))
     rng = np.random.default_rng(5)
     many = [lidar_like_cloud(int(n), KITTI["pcr"], 4, 100 + i) if n else np.zeros((0, 4), np.float32)
             for i, n in enumerate(rng.integers(0, 3000, 64))]
     many[10] = np.zeros((0, 4), np.float32)
     many[63] = lidar_like_cloud(1, KITTI["pcr"], 4, 9)
     vox64 = _voxelizer(KITTI["vs"], KITTI["pcr"], 5, 400, want_voxels, want_mean)
-    want = _host(vox64, many)
+    want = _dev(vox64, many)
     total = sum(c.shape[0] for c in many)
-    _assert_same(_dev(vox64, many), want)
+    _assert_same(_host(vox64, many), want)
     _assert_same(_dev(vox64, many, total + 777, np.nan), want)
 
 
 def test_one_graph_replays_offsets_of_any_size():
-    """One captured d3b_voxelize_dev call, replayed with 6 different offset vectors (batch 3), equals the eager
-    host-offsets call on the exactly sized points each time."""
+    """One captured d3b_voxelize_dev call, replayed with 6 different offset vectors (batch 3), equals the eager call
+    on the exactly sized points each time."""
     from det3d_b200.utils.synthetic import lidar_like_cloud
     capacity, batch = 1 << 15, 3
     vox = _voxelizer(KITTI["vs"], KITTI["pcr"], 5, 3000)
@@ -144,7 +147,7 @@ def test_one_graph_replays_offsets_of_any_size():
         graph.replay()
         got = _result(vox, out, batch)
         assert int(out["status"].item()) == 0
-        _assert_same(got, _host(ref, clouds))
+        _assert_same(got, _dev(ref, clouds))
 
 
 @pytest.mark.parametrize("raw,clamped", [
@@ -165,7 +168,7 @@ def test_malformed_offsets_set_status_and_run_clamped(raw, clamped):
     out = vox(torch.from_numpy(pts_np).cuda(), torch.tensor(raw, dtype=torch.int32, device="cuda"))
     assert int(out["status"].item()) == 1
     got = _result(vox, out, 3)
-    want = _host(ref, [pts_np[a:b] for a, b in zip(clamped[:-1], clamped[1:])])
+    want = _dev(ref, [pts_np[a:b] for a, b in zip(clamped[:-1], clamped[1:])])
     _assert_same(got, want)
     # a well-formed call on the same buffers clears the status again
     ok = vox(torch.from_numpy(pts_np).cuda(), torch.tensor(clamped, dtype=torch.int32, device="cuda"))

@@ -56,7 +56,7 @@ def run(steps, batch, n_sweep, n_sweeps, warmup, seed):
 
     def step(mode, samples):
         if mode == "per_sample":
-            clouds = [ingest_sweeps(*s) for s in samples]              # n_out.item() per sample
+            clouds = [ingest_sweeps(*s) for s in samples]              # one sync per sample
             offsets = np.cumsum([0] + [c.shape[0] for c in clouds]).tolist()
             packed = pipe.forward_graphed(torch.cat(clouds), offsets)
             if pinned_out[mode] is None:
